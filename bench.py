@@ -6,6 +6,7 @@ correspondence kernel's roofline and the CPU baseline.
 
   python bench.py --gpus N --steps K --warmup W          (torchrun for N > 1)
   python bench.py --impl reference ...                   (CPU port of the reference step)
+  python bench.py ... --dump-outputs DIR                 (rank 0 writes what the last timed step computed)
 Prints ONE JSON line on rank 0.
 """
 import argparse
@@ -48,8 +49,8 @@ def measured_peaks():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         d = json.load(open(path))
-        return d.get("bf16_tflops", 1590.0), d.get("bf16_tflops_sustained"), "measured"
-    return 1590.0, 1400.0, "fallback"
+        return d.get("bf16_tflops", 989.0), d.get("bf16_tflops_sustained"), "measured"
+    return 989.0, 989.0, "H100 SXM data sheet (dense bf16, 700 W)"
 
 
 class ClockSampler:
@@ -119,13 +120,8 @@ def k1_roofline(torch, batch=8, n=4096, kd=256, cv=3, iters=20):
     flops = batch * (2.0 * n * n * kd + 2.0 * n * n * cv)
     peak, _, src = measured_peaks()
     achieved = flops / ms / 1e9
-    traffic = None
-    summ = os.path.join(ROOT, "profiles", "k1_fwd_ncu_summary.json")
-    if os.path.exists(summ):
-        traffic = json.load(open(summ)).get("dram_bytes_per_launch")
-    return {"bound": "tensor", "kernel": "corr_fwd4_kernel (fused correlation+softmax+warp)", "achieved": achieved,
-            "peak": peak, "peak_source": src + " cuBLAS bf16 burst", "unit": "TFLOP/s", "frac": achieved / peak,
-            "frac_of_nominal_2250": achieved / 2250.0, "traffic": traffic if kd == 256 else None,
+    return {"bound": "tensor", "kernel": "corr_fwd_kernel (fused correlation+softmax+warp)", "achieved": achieved,
+            "peak": peak, "peak_source": src, "unit": "TFLOP/s", "frac": achieved / peak,
             "shape": {"batch": batch, "HW": n, "C": kd, "Cv": cv}, "ms_per_launch": ms,
             "algorithmic_flops_per_launch": flops}
 
@@ -146,9 +142,9 @@ def tapconv_roofline(torch, batch=8, hw=64, cin=512, cout=512, iters=10, device=
     be = nhwc.backend()
     algorithmic = 2.0 * batch * hw * hw * cout * cin * 9
     peak, _, src = measured_peaks()
-    out = {"bound": "tensor", "kernel": "tapconv_kernel<256> (persistent TMA + tcgen05 tap convolution)",
+    out = {"bound": "tensor", "kernel": "tapconv_kernel<256> (TMA + wgmma tap convolution)",
            "shape": {"batch": batch, "H": hw, "W": hw, "Cin": cin, "Cout": cout, "taps": 9},
-           "algorithmic_flops_per_launch": algorithmic, "peak": peak, "peak_source": src + " cuBLAS bf16 burst",
+           "algorithmic_flops_per_launch": algorithmic, "peak": peak, "peak_source": src,
            "unit": "TFLOP/s"}
     for name, split in (("single", False), ("split3", True)):
         xin = nhwc.pack(x, nhwc.F16, pad=1, split=split)
@@ -220,6 +216,36 @@ def cpu_step_images_per_sec(steps, warmup, budget_s=240.0):
     return 1.0 / (sum(timed) / len(timed)), len(timed), threads
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+DUMP_ARRAY_BYTES = 8 << 20
+
+
+def dump_outputs(torch, trainer, out_dir):
+    """What the timed step hands its caller -- every loss and every tensor of the generator's output dict -- as
+    DIR/<name>.npy in float32.  An array above 8 MB is replaced by a fixed seeded sample of its flattened elements
+    (<name>.npy) plus the sampled indices (<name>.index.npy), so that two builds compare element for element; an array
+    that would take the total past 64 MB is skipped with a warning on stderr."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"loss_" + k: v for k, v in trainer.get_latest_losses().items()}
+    arrays.update({k: v for k, v in trainer.out.items() if torch.is_tensor(v)})
+    total = 0
+    for name in sorted(arrays):
+        a = arrays[name].detach().float().reshape(-1).cpu().numpy()
+        idx = None
+        if a.nbytes > DUMP_ARRAY_BYTES:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, DUMP_ARRAY_BYTES // 8, replace=False))
+            a = a[idx]
+        size = a.nbytes + (idx.nbytes if idx is not None else 0)
+        if total + size > DUMP_LIMIT_BYTES:
+            sys.stderr.write("bench: --dump-outputs skips %s: the dump would exceed %d MB\n" % (name, DUMP_LIMIT_BYTES >> 20))
+            continue
+        total += size
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float32))
+        if idx is not None:
+            np.save(os.path.join(out_dir, name + ".index.npy"), idx.astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -233,6 +259,8 @@ def main():
                          "with the README's full flag set); 8 images per GPU in all of them")
     ap.add_argument("--stock-torch", action="store_true",
                     help="MEASUREMENT ONLY: every hand-written kernel off (reference expressions on cuDNN / cuBLAS)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's losses and generator outputs as DIR/<name>.npy")
     args = ap.parse_args()
     if args.stock_torch:
         os.environ["COCOS_STOCK_TORCH"] = "1"
@@ -335,6 +363,8 @@ def main():
     ms = timed(step_resident, args.steps)
     launches = trainer.graph_native_launches * args.steps if graphed else _lib.LAUNCHES - l0
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(torch, trainer, args.dump_outputs)
     if profile_mode:
         print(json.dumps({"profile_mode": True, "ms_per_step": ms / args.steps, "gpu_launches": launches}))
         return 0
@@ -388,7 +418,7 @@ def main():
         step_roof = None
         if args.config in (1, 4):
             ach = value / world * STEP_TFLOP_PER_IMAGE
-            step_roof = {"bound": "tensor", "achieved": ach, "peak": sustained, "peak_source": psrc + " cuBLAS bf16 sustained",
+            step_roof = {"bound": "tensor", "achieved": ach, "peak": sustained, "peak_source": psrc,
                          "unit": "TFLOP/s", "frac": ach / sustained, "per": "GPU",
                          "algorithmic_tflop_per_image": STEP_TFLOP_PER_IMAGE,
                          "note": "algorithmic FLOPs (SURVEY 8d); the default precision mode spends 3 MMAs per tap on "
@@ -396,7 +426,7 @@ def main():
         line = {"metric": METRIC, "value": value, "unit": "images/sec", "n_gpus": world,
                 "steps": args.steps, "warmup": warmup, "ms_per_step": ms / args.steps, "higher_is_better": True,
                 "scaling": "weak", "vs_baseline": None,
-                "dtype": "fp16 2-term split operands (forward, fp32 accumulate on tcgen05) on every convolution upstream "
+                "dtype": "fp16 2-term split operands (forward, fp32 accumulate on wgmma) on every convolution upstream "
                          "of warp_out / fake_image, single fp16 terms in the PatchGANs and VGG19, bf16 operands in the "
                          "backward; fp16 operands in the fused correspondence kernel",
                 "precision_mode": {"conv_precision": opt.conv_precision, "corr_precision": opt.corr_precision,
@@ -406,7 +436,7 @@ def main():
                 "config": {"workload": workload + ", full G+D train step (fwd+bwd+Adam), BASELINE configs[%d]" % args.config,
                            "global_batch": gb, "per_gpu_batch": PER_GPU_BATCH, "parallelism": "dp%d" % world,
                            "cuda_graph": graphed if trainer.graph_error is None else "capture failed: " + trainer.graph_error,
-                           "l2": "per-step activations (multi-GB) and inputs exceed the 126 MB L2; no explicit flush"},
+                           "l2": "per-step activations (multi-GB) and inputs exceed the 50 MB L2; no explicit flush"},
                 "clocks": clocks,
                 "e2e": {"value": gb * args.steps / (ms_e2e / 1e3), "unit": "images/sec", "h2d_bytes_per_step": h2d,
                         "d2h_bytes_per_step": d2h},

@@ -1,4 +1,4 @@
-"""cocosnet_b200 — B200-native (sm_100a) hot path of CoCosNet.
+"""cocosnet_b200 — H100-native (sm_90a) hot path of CoCosNet.
 
 Layout:
   csrc/            hand-written CUDA kernels + the C-ABI (libcocos_b200.so)

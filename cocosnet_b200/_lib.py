@@ -23,7 +23,7 @@ SIGNATURES = {
     "cocos_spade_mod_fwd": [_vp] * 5 + [_c_int] * 5 + [_c_float, _c_float, _c_int, _vp],
     "cocos_spade_mod_bwd": [_vp] * 7 + [_c_int] * 5 + [_c_float, _c_int, _vp],
     "cocos_cast_pitch": [_vp, _vp, ctypes.c_longlong] + [_c_int] * 6 + [_vp],
-    "cocos_conv_wgrad": [_vp, _vp, _vp] + [_c_int] * 11 + [_vp],
+    "cocos_conv_wgrad": [_vp, _vp, _vp] + [_c_int] * 11 + [_vp, _vp, _vp],
     "cocos_conv_fwd": [_vp, _vp, _vp, _vp] + [_c_int] * 10 + [_vp],
     "cocos_normalize_pack": [_vp, _vp, _vp, _vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int, _c_float, _vp],
     "cocos_normalize_pack_bwd": [_vp] * 7 + [_c_int] * 5 + [_vp],
@@ -32,6 +32,7 @@ SIGNATURES = {
     "cocos_inst_act_bwd": [_vp] * 5 + [_c_int, _c_int, _c_float, _vp],
     "cocos_tapconv": [_vp, _vp],
     "cocos_tapwgrad": [_vp, _vp],
+    "cocos_tapwgrad_workspace": [_vp, _vp],
     "cocos_pack_w": [_vp, _c_int, _c_int, _c_int, _vp, _c_int, _c_int, _c_int, _c_int, _vp, _vp, _vp, _c_int, _c_int, _vp],
     "cocos_spade_mod_nhwc_fwd": [_vp, _c_int, _c_int, _vp, _c_int, _c_int, _vp, _c_int, _c_int, _vp, _vp] + [_c_int] * 5
                                 + [_c_float, _c_float, _vp],
@@ -41,23 +42,25 @@ SIGNATURES = {
     "cocos_ctx_rows_bwd": [_vp, _vp, _vp, _c_int, _c_int, _c_int, _c_float, _c_float, _vp],
     "cocos_sn_power_iter": [_vp, _c_int, _c_int, _c_int, _vp, _vp, _vp, _c_float, _c_int, _vp],
     "cocos_pono_stats_nhwc": [_vp, _c_int, _c_int, _c_int, _c_ll, _c_float, _vp, _vp, _vp],
-    "cocos_in_stats_nhwc": [_vp, _c_int, _c_int, _c_int, _c_int, _c_int, _vp, _vp],
+    "cocos_in_stats_nhwc": [_vp, _c_int, _c_int, _c_int, _c_int, _c_int, _vp, _vp, _vp, _vp],
     "cocos_inst_act_nhwc_fwd": [_vp, _c_int, _c_int, _vp, _vp, _c_int, _c_int, _vp, _c_float, _vp, _c_int, _c_int,
                                 _c_int, _c_int, _vp, _c_int, _c_int, _c_int, _c_int, _c_int, _c_float, _vp, _c_int, _c_int,
                                 _c_int, _vp],
     "cocos_inst_act_nhwc_bwd": [_vp, _c_int, _c_int, _vp, _c_int, _vp, _c_int, _c_int, _vp, _vp, _c_int, _c_int, _vp,
                                 _c_float, _vp, _vp, _vp, _c_int, _c_int, _vp, _c_int, _c_int, _c_int, _c_int, _c_int,
-                                _c_int, _c_float, _vp, _c_int, _c_int, _vp, _c_int, _c_int, _c_int, _c_int, _vp],
+                                _c_int, _c_float, _vp, _c_int, _c_int, _vp, _c_int, _c_int, _c_int, _c_int, _vp, _vp,
+                                _vp],
     "cocos_act_bwd_nhwc": [_vp, _c_int, _vp, _c_int, _c_int, _c_int, _vp, _c_int] + [_c_int] * 5 + [_c_float, _vp],
     "cocos_nhwc_pack": [_vp, _vp] + [_c_int] * 13 + [_vp],
-    "cocos_pair_loss_nhwc_fwd": [_vp, _c_int, _vp, _c_int, _vp, _c_int, _c_ll, _c_int, _c_float, _c_int, _vp, _vp],
+    "cocos_pair_loss_nhwc_fwd": [_vp, _c_int, _vp, _c_int, _vp, _c_int, _c_ll, _c_int, _c_float, _c_int, _vp, _vp, _vp,
+                                 _vp],
     "cocos_pair_loss_nhwc_bwd": [_vp, _c_int, _vp, _c_int, _vp, _c_int, _c_ll, _c_int, _c_float, _c_int, _vp, _vp, _c_int,
                                  _c_int, _vp],
     "cocos_cast_op_bf16": [_vp, _c_int, _c_int, _vp, _c_int, _c_ll, _vp],
     "cocos_maxpool2_nhwc_fwd": [_vp, _vp] + [_c_int] * 4 + [_vp],
     "cocos_maxpool2_nhwc_bwd": [_vp, _vp, _vp] + [_c_int] * 4 + [_vp],
     "cocos_nhwc_unpack": [_vp] + [_c_int] * 8 + [_vp] + [_c_int] * 6 + [_vp],
-    "cocos_colsum_nhwc": [_vp, _c_int, _c_int, _c_int, _c_ll, _vp, _vp],
+    "cocos_colsum_nhwc": [_vp, _c_int, _c_int, _c_int, _c_ll, _vp, _vp, _vp, _vp],
     "cocos_gemm_f16": [_vp, _vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _c_ll, _c_ll, _c_ll,
                        _c_float, _c_int, _c_int, _vp],
 }
@@ -71,7 +74,7 @@ class CocosError(RuntimeError):
 
 
 def build():
-    """Compile the extension in-tree (nvcc, sm_100a)."""
+    """Compile the extension in-tree (nvcc, sm_90a)."""
     import subprocess
     subprocess.check_call(["bash", os.path.join(_HERE, "csrc", "build.sh")])
 
@@ -91,6 +94,17 @@ def lib():
         fn.restype = ctypes.c_char_p if name == "cocos_last_error" else ctypes.c_int
     _lib = h
     return h
+
+
+def call_with_workspace(fn, args, stream, what, kernels=1):
+    """fn(*args, ws, &ws_floats, stream) under the C-ABI workspace protocol: a size query (nothing launched), then the
+    call with a workspace from torch's caching allocator (stream-ordered, usable under CUDA-graph capture)."""
+    import torch
+    need = ctypes.c_longlong(0)
+    check(fn(*args, None, ctypes.byref(need), stream), what, kernels=0)
+    ws = torch.empty((max(need.value, 1),), dtype=torch.float32, device="cuda")
+    need.value = ws.numel()
+    check(fn(*args, ws.data_ptr(), ctypes.byref(need), stream), what, kernels=kernels)
 
 
 def check(rc, what, kernels=1):

@@ -2,7 +2,7 @@
 (`models.pix2pix_model`, `models.networks`, `trainers.pix2pix_trainer`,
 `options.train_options`, `options.test_options`, `util.util`): after
 `cocosnet_b200.compat.install()` those imports resolve to this package, so the
-reference's own train.py / test.py drive the B200 path unmodified apart from
+reference's own train.py / test.py drive the native path unmodified apart from
 their data loader (INTEGRATION.md)."""
 import sys
 import types

@@ -1,4 +1,4 @@
-"""Dense correspondence + warp on the fused sm_100a kernel (K1).
+"""Dense correspondence + warp on the fused sm_90a kernel (K1).
 
 Host-side mirror of the tail of NoVGGCorrespondence.forward (reference
 models/networks/correspondence.py:272-372): everything after the theta / phi
@@ -200,9 +200,9 @@ def correspondence_tail(theta_conv, phi_conv, ref_img, *, match_kernel=3, pono_c
     b, _, fh, fw = theta_conv.shape
     if precision == "auto":
         # operand rounding (2^-11 per element) reaches the logits as 100 * 2^-11 * O(1/sqrt(K)) and the softmax
-        # amplifies it by how peaked the rows are.  Measured against the reference goldens (profiles/r02_parity_*):
-        # single fp16 terms give 6.9e-4 on warp_out for the ade20k / --PONO_C features at K = 2304, but 1.0e-3 at
-        # K = 256 and 9.2-9.7e-4 for the celebahq / deepfashion features (no --PONO_C) -- too close to the 1e-3 bar.
+        # amplifies it by how peaked the rows are: against the reference goldens, single fp16 terms keep a margin to
+        # the 1e-3 bar on warp_out only for the --PONO_C features at large K (ade20k, K = 2304); at K = 256 and for the
+        # celebahq / deepfashion features (no --PONO_C) they come too close to it.
         # So single terms only where they have margin (and where the fused prologue exists); 3-term split elsewhere.
         k_total = theta_conv.shape[1] * match_kernel * match_kernel
         precision = "fp16" if (pono_c and k_total >= 1024) else "split"

@@ -1,6 +1,6 @@
 """Backward of the fused correspondence primitive (what autograd computes
-through reference correspondence.py:291-318), on the sm_100a kernels:
-stage A (csrc/corr_bwd.cu) emits dS / dS^T / P^T in bf16, three tcgen05 GEMMs
+through reference correspondence.py:291-318), on the sm_90a kernels:
+stage A (csrc/corr_bwd.cu) emits dS / dS^T / P^T in bf16, three wgmma GEMMs
 (csrc/gemm.cu) contract them with the channel-major operands."""
 import torch
 

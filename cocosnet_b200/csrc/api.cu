@@ -130,12 +130,12 @@ int cocos_cast_pitch(const float* src, void* dst, long long rows, int Win, int W
 }
 
 int cocos_conv_wgrad(const void* dy, const void* x, float* ws, int B, int H, int W, int Hin, int Win, int Cout, int Cin,
-                     int KS, int off, int dy_bf16, int x_bf16, void* stream) {
-  if (!dy || !x || !ws) {
+                     int KS, int off, int dy_bf16, int x_bf16, float* part, long long* part_floats, void* stream) {
+  if (part && (!dy || !x || !ws)) {
     set_error("conv_wgrad: null pointer");
     return -1;
   }
-  return conv_wgrad_launch(dy, x, ws, B, H, W, Hin, Win, Cout, Cin, KS, off, dy_bf16, x_bf16,
+  return conv_wgrad_launch(dy, x, ws, B, H, W, Hin, Win, Cout, Cin, KS, off, dy_bf16, x_bf16, part, part_floats,
                            static_cast<cudaStream_t>(stream));
 }
 
@@ -154,7 +154,15 @@ int cocos_tapconv(const cocos_tapconv_desc* desc, void* stream) {
 }
 
 int cocos_tapwgrad(const cocos_tapwgrad_desc* desc, void* stream) {
-  return tapwgrad_launch(desc, static_cast<cudaStream_t>(stream));
+  return tapwgrad_launch(desc, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+int cocos_tapwgrad_workspace(const cocos_tapwgrad_desc* desc, long long* floats) {
+  if (!floats) {
+    set_error("cocos_tapwgrad_workspace: null pointer argument");
+    return -1;
+  }
+  return tapwgrad_launch(desc, floats, nullptr);
 }
 
 int cocos_pack_w(const float* w, int Cout, int Cin, int KS, void* dst, int rows, int rows_alloc, int Kc, int ngroups,
@@ -219,12 +227,13 @@ int cocos_spade_mod_nhwc_bwd(const void* dy, int dy_Cs, const void* x, int x_kin
                                    dgb_Cs, B, C, H, W, pad, slope, static_cast<cudaStream_t>(stream));
 }
 
-int cocos_in_stats_nhwc(const void* x, int kind, int Cs, int B, int C, int HW, float* stats, void* stream) {
-  if (!x || !stats) {
+int cocos_in_stats_nhwc(const void* x, int kind, int Cs, int B, int C, int HW, float* stats, float* ws,
+                        long long* ws_floats, void* stream) {
+  if (ws && (!x || !stats)) {
     set_error("cocos_in_stats_nhwc: null pointer argument");
     return -1;
   }
-  return in_stats_nhwc_launch(x, kind, Cs, B, C, HW, stats, static_cast<cudaStream_t>(stream));
+  return in_stats_nhwc_launch(x, kind, Cs, B, C, HW, stats, ws, ws_floats, static_cast<cudaStream_t>(stream));
 }
 
 int cocos_inst_act_nhwc_fwd(const void* x, int x_kind, int x_Cs, const float* stats, const void* res, int res_kind,
@@ -245,15 +254,15 @@ int cocos_inst_act_nhwc_bwd(const void* dy, int dy_Cs, int dy_pad, const void* d
                             const float* slope_ptr, float slope, float* bstats, float* dslope, void* dx, int dx_Cs,
                             int dx_acc, void* dres, int dres_Cs, int dres_acc, int B, int C, int H, int W, float eps,
                             const void* gb, int gb_kind, int gb_Cs, void* dgb, int dgb_Cs, int batch_stats,
-                            int const_stats, int phase, void* stream) {
-  if (!dy || !x || !stats || !dx) {
+                            int const_stats, int phase, float* ws, long long* ws_floats, void* stream) {
+  if (ws && (!dy || !x || !stats || !dx)) {
     set_error("cocos_inst_act_nhwc_bwd: null pointer argument");
     return -1;
   }
   return inst_act_nhwc_bwd_launch(dy, dy_Cs, dy_pad, dy2, dy2_Cs, x, x_kind, x_Cs, stats, res, res_kind, res_Cs,
                                   slope_ptr, slope, bstats, dslope, dx, dx_Cs, dx_acc, dres, dres_Cs, dres_acc, B, C,
-                                  H, W, eps, gb, gb_kind, gb_Cs, dgb, dgb_Cs, batch_stats, const_stats, phase,
-                                  static_cast<cudaStream_t>(stream));
+                                  H, W, eps, gb, gb_kind, gb_Cs, dgb, dgb_Cs, batch_stats, const_stats, phase, ws,
+                                  ws_floats, static_cast<cudaStream_t>(stream));
 }
 
 int cocos_act_bwd_nhwc(const void* dy, int dy_Cs, const void* y, int y_kind, int y_Cs, int pad, void* dz, int dz_Cs,
@@ -277,12 +286,13 @@ int cocos_nhwc_pack(const float* src, void* dst, int kind, int B, int C, int Cs,
 }
 
 int cocos_pair_loss_nhwc_fwd(const void* x, int x_Cs, const void* y, int y_Cs, const float* w, int B, long long HW, int C,
-                             float scale, int mode, float* out, void* stream) {
-  if (!x || !y || !out) {
+                             float scale, int mode, float* out, float* ws, long long* ws_floats, void* stream) {
+  if (ws && (!x || !y || !out)) {
     set_error("cocos_pair_loss_nhwc_fwd: null pointer argument");
     return -1;
   }
-  return pair_loss_nhwc_fwd_launch(x, x_Cs, y, y_Cs, w, B, HW, C, scale, mode, out, static_cast<cudaStream_t>(stream));
+  return pair_loss_nhwc_fwd_launch(x, x_Cs, y, y_Cs, w, B, HW, C, scale, mode, out, ws, ws_floats,
+                                   static_cast<cudaStream_t>(stream));
 }
 
 int cocos_pair_loss_nhwc_bwd(const void* x, int x_Cs, const void* y, int y_Cs, const float* w, int B, long long HW, int C,
@@ -329,12 +339,13 @@ int cocos_nhwc_unpack(const void* src, int kind, int Cs, int c_lo, int C, int B,
                             static_cast<cudaStream_t>(stream));
 }
 
-int cocos_colsum_nhwc(const void* x, int kind, int Cs, int C, long long rows, float* out, void* stream) {
-  if (!x || !out) {
+int cocos_colsum_nhwc(const void* x, int kind, int Cs, int C, long long rows, float* out, float* ws,
+                      long long* ws_floats, void* stream) {
+  if (ws && (!x || !out)) {
     set_error("cocos_colsum_nhwc: null pointer argument");
     return -1;
   }
-  return colsum_nhwc_launch(x, kind, Cs, C, rows, out, static_cast<cudaStream_t>(stream));
+  return colsum_nhwc_launch(x, kind, Cs, C, rows, out, ws, ws_floats, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -1,4 +1,4 @@
-// K2: TMA-fed tcgen05 implicit-GEMM convolution, forward (3x3 / 1x1, stride 1), sm_100a.
+// K2: TMA-fed wgmma implicit-GEMM convolution, forward (3x3 / 1x1, stride 1), sm_90a.
 //
 //   Y[b, n, h, w] = bias[n] + sum_{r,s,c} X[b, h + r - off, w + s - off, c] * Wt[n, (r*KS + s)*Cp + c]
 //
@@ -9,10 +9,11 @@
 //     by the producer, off = 0); otherwise Hin = H and the halo is TMA out-of-bounds zero fill (off = KS/2).
 //   * the A tile of tap (r, s), channel chunk kc is ONE 4-D TMA box {64 ch, TW, TH, 1} at (kc*64, w0+s-off, h0+r-off, b):
 //     its TH*TW rows of 128 B land in (h, w) order with the 128B swizzle -- exactly the K-major operand layout of
-//     tcgen05.mma, no im2col buffer anywhere.
+//     wgmma, no im2col buffer anywhere.
 //   * B tile = weights [Cout, KS*KS*Cp] fp16 K-major, box {64, BN}.
-//   * accumulator in TMEM (fp32); epilogue adds the bias and writes NCHW fp32, coalesced along w.
-// warp 4: TMA producer, warp 5: MMA issuer (UMMA N = BN), warps 0-3: epilogue.
+//   * accumulators in registers (fp32, two warpgroups of 64 rows), staged through shared memory; the epilogue adds
+//     the bias and writes NCHW fp32, coalesced along w.
+// warp 8: TMA producer, warps 0-7: wgmma (N = BN), warps 0-3: epilogue.
 #include "corr_kernels.h"
 #include "ptx.cuh"
 #include "tmap.h"
@@ -23,7 +24,7 @@ namespace {
 
 constexpr int BM = 128, BK = 64;
 constexpr int ATOM_BYTES = 128 * BK * 2;
-constexpr int NUM_THREADS = 192;
+constexpr int NUM_THREADS = TILE_THREADS;
 
 struct ConvParams {
   int B, H, W, Cout, Cp, KS, off;
@@ -36,9 +37,6 @@ struct ConvParams {
 struct ConvBars {
   uint64_t full[6];
   uint64_t empty[6];
-  uint64_t acc_full;
-  uint32_t tmem_base;
-  uint32_t pad;
 };
 
 template <int BN>
@@ -66,25 +64,17 @@ conv_fwd_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
   if (tid == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(smem_u32(&bars->full[i]), 1);
-      mbar_init(smem_u32(&bars->empty[i]), 1);
+      mbar_init(smem_u32(&bars->empty[i]), CONSUMER_WARPS);
     }
-    mbar_init(smem_u32(&bars->acc_full), 1);
     fence_mbar_init();
   }
-  if (warp == 4 && lane == 0) {
+  if (warp == CONSUMER_WARPS && lane == 0) {
     tma_prefetch_desc(&tm_x);
     tma_prefetch_desc(&tm_w);
   }
-  if (warp == 5) {
-    tmem_alloc(smem_u32(&bars->tmem_base), BN);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = bars->tmem_base;
 
-  if (warp == 4) {
+  if (warp == CONSUMER_WARPS) {
     if (elect_one()) {
       uint32_t st = 0, ph = 0;
       for (int it = 0; it < iters; ++it) {
@@ -98,54 +88,36 @@ conv_fwd_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
         if (++st == STAGES) { st = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 5) {
-    const bool leader = elect_one();
-    const uint32_t idesc = make_idesc_f16(BM, BN, p.bf16 != 0);
-    uint32_t st = 0, ph = 0;
-    for (int it = 0; it < iters; ++it) {
-      mbar_wait(smem_u32(&bars->full[st]), ph);
-      tc_fence_after();
-      if (leader) {
-        const uint32_t a_addr = smem0 + st * STAGE_BYTES;
-        const uint64_t da = make_desc_k_sw128(a_addr), db = make_desc_k_sw128(a_addr + ATOM_BYTES);
-#pragma unroll
-        for (int s4 = 0; s4 < 4; ++s4)
-          umma_f16(tmem, desc_advance_k16(da, s4), desc_advance_k16(db, s4), idesc, (it | s4) != 0 ? 1u : 0u);
-        umma_commit(smem_u32(&bars->empty[st]));
-        if (it == iters - 1) umma_commit(smem_u32(&bars->acc_full));
-      }
-      __syncwarp();
-      if (++st == STAGES) { st = 0; ph ^= 1; }
-    }
   } else {
-    const int m = tid;  // accumulator row == pixel (th, tw) of the patch
-    const int th = m / p.TW, tw = m - th * p.TW;
-    const int h = h0 + th, w = w0 + tw;
-    const bool ok = (m < p.TH * p.TW) && h < p.H && w < p.W;
-    const uint32_t lane_sel = static_cast<uint32_t>(warp * 32) << 16;
-    mbar_wait(smem_u32(&bars->acc_full), 0);
-    tc_fence_after();
-    const size_t hw = static_cast<size_t>(p.H) * p.W;
-    float* ybase = p.y + (static_cast<size_t>(b) * p.Cout) * hw + static_cast<size_t>(h) * p.W + w;
+    float d[BN / 2];
+    const uint32_t a_off = (tid >> 7) * 64 * 128;
+    consume_stages<BN>(d, iters, STAGES, bars->full, bars->empty, p.bf16 != 0, 0,
+                       [&](uint32_t st, int k, uint64_t& da, uint64_t& db) {
+                         const uint32_t a_addr = smem0 + st * STAGE_BYTES;
+                         da = desc_advance_k16(make_desc_k_sw128(a_addr + a_off), k);
+                         db = desc_advance_k16(make_desc_k_sw128(a_addr + ATOM_BYTES), k);
+                       });
+    const float* tile = stage_acc<BN>(d, smem_gen);
+    if (warp < 4) {
+      const int m = tid;  // accumulator row == pixel (th, tw) of the patch
+      const int th = m / p.TW, tw = m - th * p.TW;
+      const int h = h0 + th, w = w0 + tw;
+      const bool ok = (m < p.TH * p.TW) && h < p.H && w < p.W;
+      const size_t hw = static_cast<size_t>(p.H) * p.W;
+      float* ybase = p.y + (static_cast<size_t>(b) * p.Cout) * hw + static_cast<size_t>(h) * p.W + w;
 #pragma unroll 1
-    for (int c = 0; c < BN / 32; ++c) {
-      uint32_t r[32];
-      tmem_ld32(tmem + lane_sel + c * 32, r);
-      tmem_wait_ld();
-      if (ok) {
+      for (int c = 0; c < BN / 32; ++c) {
+        uint32_t r[32];
+        acc_ld32(tile + m * (BN + 4) + c * 32, r);
+        if (ok) {
 #pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const int n = n0 + c * 32 + i;
-          if (n < p.Cout) ybase[static_cast<size_t>(n) * hw] = __uint_as_float(r[i]) + (p.bias ? p.bias[n] : 0.f);
+          for (int i = 0; i < 32; ++i) {
+            const int n = n0 + c * 32 + i;
+            if (n < p.Cout) ybase[static_cast<size_t>(n) * hw] = __uint_as_float(r[i]) + (p.bias ? p.bias[n] : 0.f);
+          }
         }
       }
     }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc(tmem, BN);
   }
 }
 

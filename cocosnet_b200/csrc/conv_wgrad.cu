@@ -1,21 +1,22 @@
-// K2w: TMA-fed tcgen05 implicit-GEMM convolution, backward-weights (3x3 / 1x1, stride 1), sm_100a.
+// K2w: TMA-fed wgmma implicit-GEMM convolution, backward-weights (3x3 / 1x1, stride 1), sm_90a.
 //
 //   dW[n, c, r, s] = sum_{b,h,w} dY[b, n, h, w] * X[b, c, h + r - off, w + s - off]
 //
 // One GEMM per filter tap: M = 128 output channels n, N = 128/256 input channels c, K = the B*H*W output pixels.
 // Both operands are K-major with K = pixels, which is exactly what NCHW gives for free:
 //   * A tile = dY, 16-bit NCHW [B, Cout, H, Wp]: one 4-D TMA box {bw, bh, 128, 1} = 64 pixels (bh rows of bw) of 128
-//     channels; each channel's 64 pixels land as one 128-byte swizzled row -- the tcgen05 K-major layout.
+//     channels; each channel's 64 pixels land as one 128-byte swizzled row -- the wgmma K-major layout.
 //   * B tile = X, 16-bit [KS][B, Cin, Hin, Wp]: KS column-shifted NCHW copies (copy s holds columns s-off .. s-off+W-1;
 //     a TMA box has to start on a 16-byte boundary of the innermost dimension, so the tap's column shift is baked into
 //     the copy and only the row shift is a coordinate): box {bw, bh, BN, 1} at (w0, h0 + r - off, c0, s*B + b).
 //     Rows outside the image and ragged edges are TMA out-of-bounds zero fill (a pixel that does not exist has
 //     dY == 0 from the same fill, so it contributes nothing).
 //   * Wp: row pitch rounded up to 8 elements (TMA needs 16-byte strides); cocos_cast_pitch makes all these copies.
-//   * the pixel range is split over gridDim.z (split-K) so that every layer fills the 148 SMs; partial tiles are added
-//     into ws[tap][c][n] (fp32, n contiguous -> coalesced red.global.add), which the host permutes to [n][c][r][s].
-// dY is bf16 (gradient range), X fp16 or bf16 (instruction descriptor carries the two formats separately).
-// warp 4: TMA producer, warp 5: MMA issuer, warps 0-3: epilogue.
+//   * the pixel range is split over gridDim.z (split-K) so that every layer fills the SMs; split k stores its
+//     partial tile into slice k of a workspace and ordered_sum() adds the slices in split order into ws[tap][c][n]
+//     (fp32, n contiguous), which the host permutes to [n][c][r][s].
+// dY is bf16 (gradient range) and X must have the same 16-bit format (wgmma takes one operand type).
+// warp 8: TMA producer, warps 0-7: wgmma, warps 0-3: epilogue.
 #include <cstdlib>
 
 #include <cuda_bf16.h>
@@ -31,7 +32,7 @@ namespace {
 
 constexpr int BM = 128, BK = 64;
 constexpr int ATOM_BYTES = 128 * BK * 2;
-constexpr int NUM_THREADS = 192;
+constexpr int NUM_THREADS = TILE_THREADS;
 
 struct WgradParams {
   int B, H, W, Cout, Cin, KS, off;
@@ -39,21 +40,14 @@ struct WgradParams {
   int total_chunks, chunks_per_split, splits;
   int a_bf16, b_bf16;
   int dbg;  // COCOS_WG_DBG bring-up knock-outs: 1 no x load, 2 no dy load, 4 no MMA, 8 no stores
-  float* ws;  // [KS*KS, Cin, Cout]
+  float* ws;  // [KS*KS, Cin, Cout], or with splits > 1 the workspace [splits][KS*KS, Cin, Cout]
+  long long ws_size;
 };
 
 struct WgradBars {
   uint64_t full[6];
   uint64_t empty[6];
-  uint64_t acc_full;
-  uint32_t tmem_base;
-  uint32_t pad;
 };
-
-__host__ __device__ constexpr uint32_t make_idesc_mixed(int m, int n, bool a_bf16, bool b_bf16) {
-  return (1u << 4) | ((a_bf16 ? 1u : 0u) << 7) | ((b_bf16 ? 1u : 0u) << 10) | (static_cast<uint32_t>(n >> 3) << 17) |
-         (static_cast<uint32_t>(m >> 4) << 24);
-}
 
 template <int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
@@ -79,25 +73,17 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tm_dy, const __grid_consta
   if (tid == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(smem_u32(&bars->full[i]), 1);
-      mbar_init(smem_u32(&bars->empty[i]), 1);
+      mbar_init(smem_u32(&bars->empty[i]), CONSUMER_WARPS);
     }
-    mbar_init(smem_u32(&bars->acc_full), 1);
     fence_mbar_init();
   }
-  if (warp == 4 && lane == 0) {
+  if (warp == CONSUMER_WARPS && lane == 0) {
     tma_prefetch_desc(&tm_dy);
     tma_prefetch_desc(&tm_x);
   }
-  if (warp == 5) {
-    tmem_alloc(smem_u32(&bars->tmem_base), BN);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = bars->tmem_base;
 
-  if (warp == 4) {
+  if (warp == CONSUMER_WARPS) {
     if (elect_one()) {
       uint32_t st = 0, ph = 0;
       int chunk = chunk_lo;
@@ -119,57 +105,47 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tm_dy, const __grid_consta
         }
       }
     }
-  } else if (warp == 5) {
-    const bool leader = elect_one();
-    const uint32_t idesc = make_idesc_mixed(BM, BN, p.a_bf16 != 0, p.b_bf16 != 0);
-    uint32_t st = 0, ph = 0;
-    for (int it = 0; it < iters; ++it) {
-      mbar_wait(smem_u32(&bars->full[st]), ph);
-      tc_fence_after();
-      if (leader) {
-        const uint32_t a_addr = smem0 + st * STAGE_BYTES;
-        const uint64_t da = make_desc_k_sw128(a_addr), db = make_desc_k_sw128(a_addr + ATOM_BYTES);
-        if (!(p.dbg & 4)) {
-#pragma unroll
-          for (int s4 = 0; s4 < 4; ++s4)
-            umma_f16(tmem, desc_advance_k16(da, s4), desc_advance_k16(db, s4), idesc, (it | s4) != 0 ? 1u : 0u);
-        }
-        umma_commit(smem_u32(&bars->empty[st]));
-        if (it == iters - 1) umma_commit(smem_u32(&bars->acc_full));
-      }
-      __syncwarp();
-      if (++st == STAGES) { st = 0; ph ^= 1; }
-    }
   } else {
-    const int n = n0 + tid;  // accumulator row == output channel
-    const uint32_t lane_sel = static_cast<uint32_t>(warp * 32) << 16;
-    mbar_wait(smem_u32(&bars->acc_full), 0);
-    tc_fence_after();
-    float* wbase = p.ws + (static_cast<size_t>(tap) * p.Cin) * p.Cout + n;
-    const bool plain = p.splits == 1;
-#pragma unroll 1
-    for (int cc = 0; cc < BN / 32; ++cc) {
-      uint32_t v[32];
-      tmem_ld32(tmem + lane_sel + cc * 32, v);
-      tmem_wait_ld();
-      if (n < p.Cout && !(p.dbg & 8)) {
+    float d[BN / 2];
+    const uint32_t a_off = (tid >> 7) * 64 * 128;
+    if (p.dbg & 4) {
 #pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const int c = c0 + cc * 32 + i;
-          if (c < p.Cin) {
-            float* dst = wbase + static_cast<size_t>(c) * p.Cout;
-            if (plain) *dst = __uint_as_float(v[i]);
-            else atomicAdd(dst, __uint_as_float(v[i]));
+      for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+    }
+    consume_stages<BN>(d, (p.dbg & 4) ? 0 : iters, STAGES, bars->full, bars->empty, p.a_bf16 != 0, 0,
+                       [&](uint32_t st, int k, uint64_t& da, uint64_t& db) {
+                         const uint32_t a_addr = smem0 + st * STAGE_BYTES;
+                         da = desc_advance_k16(make_desc_k_sw128(a_addr + a_off), k);
+                         db = desc_advance_k16(make_desc_k_sw128(a_addr + ATOM_BYTES), k);
+                       });
+    if (p.dbg & 4) {  // no MMA: the stages still have to be released for the producer
+      uint32_t st = 0, ph = 0;
+      for (int it = 0; it < iters; ++it) {
+        mbar_wait(smem_u32(&bars->full[st]), ph);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(smem_u32(&bars->empty[st]));
+        if (++st == STAGES) { st = 0; ph ^= 1; }
+      }
+    }
+    const float* tile = stage_acc<BN>(d, smem_gen);
+    if (warp < 4) {
+      const int n = n0 + tid;  // accumulator row == output channel
+      float* wbase = p.ws + split * p.ws_size + (static_cast<size_t>(tap) * p.Cin) * p.Cout + n;
+#pragma unroll 1
+      for (int cc = 0; cc < BN / 32; ++cc) {
+        uint32_t v[32];
+        acc_ld32(tile + tid * (BN + 4) + cc * 32, v);
+        if (n < p.Cout && !(p.dbg & 8)) {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) {
+            const int c = c0 + cc * 32 + i;
+            if (c < p.Cin) {
+              wbase[static_cast<size_t>(c) * p.Cout] = __uint_as_float(v[i]);
+            }
           }
         }
       }
     }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc(tmem, BN);
   }
 }
 
@@ -210,7 +186,7 @@ int cast_pitch_launch(const float* src, void* dst, long long rows, int Win, int 
   }
   const long long total = rows * ((Wout + 3) / 4);
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > num_sms() * 16ll) blocks = num_sms() * 16ll;
   cast_pitch_kernel<<<static_cast<int>(blocks), 256, 0, stream>>>(src, static_cast<uint16_t*>(dst), rows, Win, Wout, Wp,
                                                                   nshift, off, bf16);
   COCOS_CUDA_CHECK(cudaGetLastError());
@@ -218,7 +194,8 @@ int cast_pitch_launch(const float* src, void* dst, long long rows, int Win, int 
 }
 
 int conv_wgrad_launch(const void* dy, const void* x, float* ws, int B, int H, int W, int Hin, int Win, int Cout, int Cin,
-                      int KS, int off, int a_bf16, int b_bf16, cudaStream_t stream) {
+                      int KS, int off, int a_bf16, int b_bf16, float* ws_part, long long* ws_floats,
+                      cudaStream_t stream) {
   if (B <= 0 || H <= 0 || W <= 0 || Hin <= 0 || Win <= 0 || Cout <= 0 || Cin <= 0 || (KS != 1 && KS != 3) || off < 0 ||
       off >= KS) {
     set_error("conv_wgrad: bad shape (B=%d H=%d W=%d Hin=%d Win=%d Cout=%d Cin=%d KS=%d off=%d)", B, H, W, Hin, Win,
@@ -230,7 +207,7 @@ int conv_wgrad_launch(const void* dy, const void* x, float* ws, int B, int H, in
   int bw = 8;
   while (bw < W && bw < 64) bw *= 2;
   if (bw < 64) {
-    // a {bw < 64, bh, C, 1} box does not land as dense 128-byte swizzled rows (measured: illegal address on B200), so
+    // a {bw < 64, bh, C, 1} box does not land as dense 128-byte swizzled rows, so
     // narrow layers are not taken here; the host routes them to the library wgrad.
     set_error("conv_wgrad: W=%d < 64 is not supported", W);
     return -1;
@@ -239,6 +216,10 @@ int conv_wgrad_launch(const void* dy, const void* x, float* ws, int B, int H, in
   p.chunks_w = (W + bw - 1) / bw;
   p.chunks_h = (H + p.bh - 1) / p.bh;
   p.total_chunks = B * p.chunks_h * p.chunks_w;
+  if (a_bf16 != b_bf16) {
+    set_error("conv_wgrad: dY and X must share one 16-bit format (a_bf16=%d b_bf16=%d)", a_bf16, b_bf16);
+    return -1;
+  }
   p.a_bf16 = a_bf16; p.b_bf16 = b_bf16;
   {
     const char* e = getenv("COCOS_WG_DBG");
@@ -247,14 +228,17 @@ int conv_wgrad_launch(const void* dy, const void* x, float* ws, int B, int H, in
   p.ws = ws;
   const int BN = Cin > 128 ? 256 : 128;
   const int mt = (Cout + BM - 1) / BM, nt = (Cin + BN - 1) / BN, taps = KS * KS;
-  // split-K: aim at ~2 waves of 148 CTAs, keep >= 8 chunks (512 pixels) per CTA so the prologue/epilogue amortise
-  int splits = (2 * 148 + mt * nt * taps - 1) / (mt * nt * taps);
+  // split-K: aim at ~2 waves of CTAs, keep >= 8 chunks (512 pixels) per CTA so the prologue/epilogue amortise
+  int splits = (2 * num_sms() + mt * nt * taps - 1) / (mt * nt * taps);
   const int max_splits = (p.total_chunks + 7) / 8;
   if (splits > max_splits) splits = max_splits;
   if (splits < 1) splits = 1;
   p.chunks_per_split = (p.total_chunks + splits - 1) / splits;
   p.splits = (p.total_chunks + p.chunks_per_split - 1) / p.chunks_per_split;  // no empty CTA
-  if (p.splits > 1) COCOS_CUDA_CHECK(cudaMemsetAsync(ws, 0, sizeof(float) * taps * Cin * Cout, stream));
+  p.ws_size = (long long)taps * Cin * Cout;
+  const int wc = workspace_check(ws_part, ws_floats, p.splits > 1 ? p.splits * p.ws_size : 0, "conv_wgrad");
+  if (wc) return wc < 0 ? -1 : 0;
+  if (p.splits > 1) p.ws = ws_part;
 
   const int Wp = (W + 7) / 8 * 8;
   (void)Win;
@@ -284,6 +268,7 @@ int conv_wgrad_launch(const void* dy, const void* x, float* ws, int B, int H, in
     conv_wgrad_kernel<128><<<grid, NUM_THREADS, smem_bytes, stream>>>(tm_dy, tm_x, p);
   }
   COCOS_CUDA_CHECK(cudaGetLastError());
+  if (p.splits > 1) return ordered_sum(p.ws, p.splits, p.ws_size, ws, 0, stream);
   return 0;
 }
 

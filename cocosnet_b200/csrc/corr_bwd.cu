@@ -4,14 +4,14 @@
 //     dP = dO V^T,  D[i] = sum_c dO[c,i] O[c,i]
 // as bf16 (dO enters row-scaled in fp16, the scale is divided back out) in BOTH
 // orientations -- dS [B,Nq,Nkp] and dS^T [B,Nk,Nqp] -- plus optionally P^T.
-// Two plain tcgen05 GEMMs (gemm.cu) then give dQ^T = K^T-major x dS and
+// Two plain wgmma GEMMs (gemm.cu) then give dQ^T = K^T-major x dS and
 // dK^T = Q^T-major x dS^T; a third gives dV from P^T.  This is what autograd
 // does through reference correspondence.py:291-318, without keeping the three
 // fp32 N x N tensors alive.
 //
-// CTA = 128 query rows, streams 128-key tiles.  warp 4: TMA, warp 5: MMA
-// (S and dP, both double-buffered in TMEM: 4 x 128 columns), warps 0-3: one
-// thread per query row.
+// CTA = 128 query rows, streams 128-key tiles.  warp 8: TMA, warps 0-7: two
+// warpgroups of 64 query rows; S and dP by wgmma into registers, the softmax
+// Jacobian on the accumulator fragments, dS staged through one smem tile.
 #include "corr_kernels.h"
 #include "ptx.cuh"
 #include "tmap.h"
@@ -24,7 +24,8 @@ namespace {
 
 constexpr int BM = 128, BN = 128, BK = 64;
 constexpr int ATOM_BYTES = 128 * BK * 2;
-constexpr int NUM_THREADS = 192;
+constexpr int NUM_THREADS = 32 * CONSUMER_WARPS + 32;
+constexpr int CT = 32 * CONSUMER_WARPS;  // consumer threads
 constexpr int MAX_STAGES = 4;
 constexpr int TPITCH = 136;                     // staging tile pitch (fp16 elements)
 constexpr int TILE_BYTES = 128 * TPITCH * 2;    // 34816
@@ -49,13 +50,9 @@ struct BwdBars {
   uint64_t k_empty[MAX_STAGES];
   uint64_t v_full;
   uint64_t v_empty;
-  uint64_t sdp_full[2];
-  uint64_t sdp_empty[2];
-  uint32_t tmem_base;
-  uint32_t pad;
 };
 
-__device__ __forceinline__ void wg_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
+__device__ __forceinline__ void wg_sync() { bar_sync(1, CT); }
 
 // copy a staged 128x128 fp16 tile (pitch TPITCH) to global rows of pitch `gpitch`
 __device__ __forceinline__ uint32_t pack_bf2(float lo, float hi) {
@@ -68,8 +65,8 @@ __device__ __forceinline__ void copy_tile_out(const uint8_t* tile, uint16_t* gba
   const int chunk = tid & 15;
   if (chunk * 8 >= valid_cols) return;
 #pragma unroll 4
-  for (int it = 0; it < 16; ++it) {
-    const int r = (tid >> 4) + it * 8;
+  for (int it = 0; it < 128 / (CT / 16); ++it) {
+    const int r = (tid >> 4) + it * (CT / 16);
     if (r < valid_rows) {
       const uint4 v = *reinterpret_cast<const uint4*>(tile + (r * TPITCH + chunk * 8) * 2);
       *reinterpret_cast<uint4*>(gbase + static_cast<size_t>(r) * gpitch + chunk * 8) = v;
@@ -102,32 +99,21 @@ corr_bwd_ds_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
     mbar_init(smem_u32(&bars->do_full), 1);
     for (int i = 0; i < p.ns; ++i) {
       mbar_init(smem_u32(&bars->k_full[i]), 1);
-      mbar_init(smem_u32(&bars->k_empty[i]), 1);
+      mbar_init(smem_u32(&bars->k_empty[i]), CONSUMER_WARPS);
     }
     mbar_init(smem_u32(&bars->v_full), 1);
-    mbar_init(smem_u32(&bars->v_empty), 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(smem_u32(&bars->sdp_full[i]), 1);
-      mbar_init(smem_u32(&bars->sdp_empty[i]), 128);
-    }
+    mbar_init(smem_u32(&bars->v_empty), CONSUMER_WARPS);
     fence_mbar_init();
   }
-  if (warp == 4 && lane == 0) {
+  if (warp == CONSUMER_WARPS && lane == 0) {
     tma_prefetch_desc(&tm_q);
     tma_prefetch_desc(&tm_k);
     tma_prefetch_desc(&tm_do);
     tma_prefetch_desc(&tm_v);
   }
-  if (warp == 5) {
-    tmem_alloc(smem_u32(&bars->tmem_base), 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = bars->tmem_base;  // S0 [0,128) S1 [128,256) dP0 [256,384) dP1 [384,512)
 
-  if (warp == 4) {
+  if (warp == CONSUMER_WARPS) {
     if (lane == 0) {
       mbar_expect_tx(smem_u32(&bars->do_full), op_bytes);
       for (int vc = 0; vc < p.vc_count; ++vc)
@@ -149,125 +135,110 @@ corr_bwd_ds_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
       }
     }
     __syncwarp();
-  } else if (warp == 5) {
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_f16(BM, BN);
-      uint32_t ks = 0, kph = 0;
-      mbar_wait(smem_u32(&bars->do_full), 0);
-      for (int t = 0; t < T; ++t) {
-        const int b = t & 1;
-        if (t >= 2) mbar_wait(smem_u32(&bars->sdp_empty[b]), ((t >> 1) - 1) & 1);
-        tc_fence_after();
-        for (int kc = 0; kc < p.kc_count; ++kc) {
-          mbar_wait(smem_u32(&bars->k_full[ks]), kph);
-          tc_fence_after();
-          const uint32_t a_addr = k_ring + ks * stage_bytes;
-          const uint32_t b_addr = a_addr + ATOM_BYTES;
+    return;
+  }
+
+  const int wg = tid >> 7, t = tid & 127;
+  const int r0 = 64 * wg + 16 * (t >> 5) + ((t & 31) >> 2);  // fragment rows r0, r0 + 8
+  const int cq = 2 * (t & 3);
+  const uint32_t a_off = wg * 64 * 128;
+  const float c2 = p.scale_log2;
+  // D'[i] = sum_c dO'[i,c] * O[c,i] with the SAME fp16-rounded, row-scaled dO' the dP MMA consumes, so
+  // that sum_j P[i,j] (dP'[i,j] - D'[i]) cancels to rounding noise instead of to an fp16-vs-fp32 bias.
+  float lse2[2], dsum[2], gs[2];
 #pragma unroll
-          for (int s4 = 0; s4 < 4; ++s4)
-            umma_f16(tmem + b * BN, make_desc_k_sw128(a_addr + s4 * 32), make_desc_k_sw128(b_addr + s4 * 32), idesc,
-                     (kc | s4) != 0 ? 1u : 0u);
-          umma_commit(smem_u32(&bars->k_empty[ks]));
-          if (++ks == static_cast<uint32_t>(p.ns)) { ks = 0; kph ^= 1; }
-        }
-        mbar_wait(smem_u32(&bars->v_full), t & 1);
-        tc_fence_after();
-        for (int vc = 0; vc < p.vc_count; ++vc) {
-#pragma unroll
-          for (int s4 = 0; s4 < 4; ++s4)
-            umma_f16(tmem + 256 + b * BN, make_desc_k_sw128(do_smem + vc * ATOM_BYTES + s4 * 32),
-                     make_desc_k_sw128(v_smem + vc * ATOM_BYTES + s4 * 32), idesc, (vc | s4) != 0 ? 1u : 0u);
-        }
-        umma_commit(smem_u32(&bars->v_empty));
-        umma_commit(smem_u32(&bars->sdp_full[b]));
-      }
-    }
-    __syncwarp();
-  } else {
-    const int row = tid;
-    const int q = q0 + row;
-    const bool row_ok = q < p.Nq;
-    const uint32_t lane_sel = static_cast<uint32_t>(warp * 32) << 16;
-    const float c2 = p.scale_log2;
-    // D'[i] = sum_c dO'[i,c] * O[c,i] with the SAME fp16-rounded, row-scaled dO' the dP MMA consumes, so
-    // that sum_j P[i,j] (dP'[i,j] - D'[i]) cancels to rounding noise instead of to an fp16-vs-fp32 bias.
-    float lse2 = INFINITY, dsum = 0.f, gs = 0.f;
-    if (row_ok) {
-      lse2 = p.lse[static_cast<size_t>(bidx) * p.Nq + q] * 1.4426950408889634f;
+  for (int r = 0; r < 2; ++r) {
+    const int q = q0 + r0 + 8 * r;
+    lse2[r] = INFINITY; dsum[r] = 0.f; gs[r] = 0.f;
+    if (q < p.Nq) {
+      lse2[r] = p.lse[static_cast<size_t>(bidx) * p.Nq + q] * 1.4426950408889634f;
       const __half* drow = p.do16 + (static_cast<size_t>(bidx) * p.Nq + q) * p.Cvk;
       for (int c = 0; c < p.Cv; ++c)
-        dsum = fmaf(__half2float(drow[c]), p.out[(static_cast<size_t>(bidx) * p.Cv + c) * p.Nq + q], dsum);
-      gs = p.scale / p.rscale[static_cast<size_t>(bidx) * p.Nq + q];  // undo the row scale: true dS in bf16
-    }
-    const int valid_rows = min(BM, p.Nq - q0);
-
-    for (int j = 0; j < T; ++j) {
-      const int b = j & 1;
-      const int valid_cols = min(BN, p.Nk - j * BN);
-      mbar_wait(smem_u32(&bars->sdp_full[b]), (j >> 1) & 1);
-      tc_fence_after();
-      float s[BN];
-#pragma unroll
-      for (int c = 0; c < 4; ++c)
-        tmem_ld32(tmem + lane_sel + b * BN + c * 32, reinterpret_cast<uint32_t*>(&s[c * 32]));
-      tmem_wait_ld();
-#pragma unroll
-      for (int c = 0; c < BN; ++c) {
-        const float pv = ex2(fmaf(s[c], c2, -lse2));
-        s[c] = (c < valid_cols) ? pv : 0.f;
-      }
-      uint32_t dsp[BN / 2];
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t r[32];
-        tmem_ld32(tmem + lane_sel + 256 + b * BN + c * 32, r);
-        tmem_wait_ld();
-#pragma unroll
-        for (int i = 0; i < 32; i += 2) {
-          const float d0 = s[c * 32 + i] * (__uint_as_float(r[i]) - dsum) * gs;
-          const float d1 = s[c * 32 + i + 1] * (__uint_as_float(r[i + 1]) - dsum) * gs;
-          dsp[(c * 32 + i) >> 1] = pack_bf2(d0, d1);
-        }
-      }
-      tc_fence_before();
-      mbar_arrive(smem_u32(&bars->sdp_empty[b]));
-
-      // stage dS row-major, then transposed, (then P^T) through one smem tile
-#pragma unroll
-      for (int c = 0; c < 16; ++c)
-        *reinterpret_cast<uint4*>(tile + (row * TPITCH + c * 8) * 2) =
-            make_uint4(dsp[4 * c], dsp[4 * c + 1], dsp[4 * c + 2], dsp[4 * c + 3]);
-      wg_sync();
-      copy_tile_out(tile, p.ds + (static_cast<size_t>(bidx) * p.Nq + q0) * p.Nkp + j * BN, p.Nkp, valid_rows,
-                    valid_cols, tid);
-      wg_sync();
-#pragma unroll
-      for (int c = 0; c < BN / 2; ++c) {
-        *reinterpret_cast<uint16_t*>(tile + ((2 * c) * TPITCH + row) * 2) = static_cast<uint16_t>(dsp[c] & 0xFFFF);
-        *reinterpret_cast<uint16_t*>(tile + ((2 * c + 1) * TPITCH + row) * 2) = static_cast<uint16_t>(dsp[c] >> 16);
-      }
-      wg_sync();
-      copy_tile_out(tile, p.dst + (static_cast<size_t>(bidx) * p.Nk + j * BN) * p.Nqp + q0, p.Nqp, valid_cols,
-                    valid_rows, tid);
-      wg_sync();
-      if (p.pt != nullptr) {
-#pragma unroll
-        for (int c = 0; c < BN / 2; ++c) {
-          const uint32_t h = pack_bf2(s[2 * c], s[2 * c + 1]);
-          *reinterpret_cast<uint16_t*>(tile + ((2 * c) * TPITCH + row) * 2) = static_cast<uint16_t>(h & 0xFFFF);
-          *reinterpret_cast<uint16_t*>(tile + ((2 * c + 1) * TPITCH + row) * 2) = static_cast<uint16_t>(h >> 16);
-        }
-        wg_sync();
-        copy_tile_out(tile, p.pt + (static_cast<size_t>(bidx) * p.Nk + j * BN) * p.Nqp + q0, p.Nqp, valid_cols,
-                      valid_rows, tid);
-        wg_sync();
-      }
+        dsum[r] = fmaf(__half2float(drow[c]), p.out[(static_cast<size_t>(bidx) * p.Cv + c) * p.Nq + q], dsum[r]);
+      gs[r] = p.scale / p.rscale[static_cast<size_t>(bidx) * p.Nq + q];  // undo the row scale: true dS in bf16
     }
   }
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 512);
+  const int valid_rows = min(BM, p.Nq - q0);
+  mbar_wait(smem_u32(&bars->do_full), 0);
+
+  uint32_t ks = 0, kph = 0;
+  for (int j = 0; j < T; ++j) {
+    const int valid_cols = min(BN, p.Nk - j * BN);
+    float s[BN / 2], dp[BN / 2];
+    for (int kc = 0; kc < p.kc_count; ++kc) {
+      mbar_wait_quiet(smem_u32(&bars->k_full[ks]), kph);
+      const uint32_t a_addr = k_ring + ks * stage_bytes;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_ss<BN, false>(s, desc_advance_k16(make_desc_k_sw128(a_addr + a_off), k),
+                            desc_advance_k16(make_desc_k_sw128(a_addr + ATOM_BYTES), k), (kc | k) != 0 ? 1 : 0, 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(smem_u32(&bars->k_empty[ks]));
+      if (++ks == static_cast<uint32_t>(p.ns)) { ks = 0; kph ^= 1; }
+    }
+    mbar_wait_quiet(smem_u32(&bars->v_full), j & 1);
+    wgmma_fence();
+    for (int vc = 0; vc < p.vc_count; ++vc) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_ss<BN, false>(dp, desc_advance_k16(make_desc_k_sw128(do_smem + vc * ATOM_BYTES + a_off), k),
+                            desc_advance_k16(make_desc_k_sw128(v_smem + vc * ATOM_BYTES), k), (vc | k) != 0 ? 1 : 0, 0);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(smem_u32(&bars->v_empty));
+
+    // fragment element i: row r0 + 8 * ((i >> 1) & 1), column 8 * (i >> 2) + cq + (i & 1)
+    uint32_t dsp[BN / 4];  // bf16 pairs (i, i + 1) for even i
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) {
+      const int r = (i >> 1) & 1, col = 8 * (i >> 2) + cq + (i & 1);
+      const float pv = ex2(fmaf(s[i], c2, -lse2[r]));
+      s[i] = (col < valid_cols) ? pv : 0.f;
+    }
+#pragma unroll
+    for (int i = 0; i < BN / 2; i += 2) {
+      const int r = (i >> 1) & 1;
+      dsp[i >> 1] = pack_bf2(s[i] * (dp[i] - dsum[r]) * gs[r], s[i + 1] * (dp[i + 1] - dsum[r]) * gs[r]);
+    }
+
+    // stage dS row-major, then transposed, (then P^T) through one smem tile
+#pragma unroll
+    for (int i = 0; i < BN / 2; i += 2) {
+      const int row = r0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + cq;
+      *reinterpret_cast<uint32_t*>(tile + (row * TPITCH + col) * 2) = dsp[i >> 1];
+    }
+    wg_sync();
+    copy_tile_out(tile, p.ds + (static_cast<size_t>(bidx) * p.Nq + q0) * p.Nkp + j * BN, p.Nkp, valid_rows,
+                  valid_cols, tid);
+    wg_sync();
+#pragma unroll
+    for (int i = 0; i < BN / 2; i += 2) {
+      const int row = r0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + cq;
+      *reinterpret_cast<uint16_t*>(tile + (col * TPITCH + row) * 2) = static_cast<uint16_t>(dsp[i >> 1] & 0xFFFF);
+      *reinterpret_cast<uint16_t*>(tile + ((col + 1) * TPITCH + row) * 2) = static_cast<uint16_t>(dsp[i >> 1] >> 16);
+    }
+    wg_sync();
+    copy_tile_out(tile, p.dst + (static_cast<size_t>(bidx) * p.Nk + j * BN) * p.Nqp + q0, p.Nqp, valid_cols,
+                  valid_rows, tid);
+    wg_sync();
+    if (p.pt != nullptr) {
+#pragma unroll
+      for (int i = 0; i < BN / 2; i += 2) {
+        const int row = r0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + cq;
+        const uint32_t h = pack_bf2(s[i], s[i + 1]);
+        *reinterpret_cast<uint16_t*>(tile + (col * TPITCH + row) * 2) = static_cast<uint16_t>(h & 0xFFFF);
+        *reinterpret_cast<uint16_t*>(tile + ((col + 1) * TPITCH + row) * 2) = static_cast<uint16_t>(h >> 16);
+      }
+      wg_sync();
+      copy_tile_out(tile, p.pt + (static_cast<size_t>(bidx) * p.Nk + j * BN) * p.Nqp + q0, p.Nqp, valid_cols,
+                    valid_rows, tid);
+      wg_sync();
+    }
   }
 }
 

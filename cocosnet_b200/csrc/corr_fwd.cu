@@ -1,4 +1,4 @@
-// K1: fused correlation -> softmax -> warp for sm_100a.
+// K1: fused correlation -> softmax -> warp for sm_90a.
 //
 //   O[b,c,i] = sum_j softmax_j(scale * <Q[b,i,:], K[b,j,:]>) * V[b,j,c]
 //
@@ -6,13 +6,13 @@
 // (/temperature), :307 (row softmax) and :318/:334 (matmul with the exemplar /
 // its mask) without ever writing the HWxHW matrix to HBM.
 //
-// One CTA owns 128 query rows and streams 128-key tiles:
-//   warp 4  : TMA producer  (Q once or chunk-streamed, K chunks, V tiles)
-//   warp 5  : tcgen05.mma issuer (S = Q K^T into a double-buffered TMEM tile,
-//             O += P V into a TMEM accumulator), TMEM owner
-//   warps 0-3: online softmax, one thread per query row (TMEM lane): S from
-//             TMEM -> registers, exp2, P as fp16 into 128B-swizzled smem (the A
-//             operand of the second MMA), lazy rescale of O, final epilogue.
+// One CTA owns 128 query rows and streams 64-key tiles:
+//   warp 8   : TMA producer (Q once or chunk-streamed, K chunks, V tiles)
+//   warps 0-7: two warpgroups of 64 query rows each.  S = Q K^T by wgmma into registers, online softmax on the
+//              accumulator fragments (row max / sum over the 4 threads sharing a row), then
+//              * PVN > 0: O += P V by wgmma with P as the fp16 register operand (O in registers, N = PVN >= Cvp);
+//              * CV > 0 (Cv <= 4 value channels, fp32 V): P V on the CUDA cores inside the exp loop, P and V stay
+//                fp32 (no fp16 rounding of the probabilities).
 #include "corr_kernels.h"
 #include "ptx.cuh"
 #include "tmap.h"
@@ -24,20 +24,21 @@ namespace cocos {
 namespace {
 
 constexpr int BM = 128;  // queries per CTA
-constexpr int BN = 128;  // keys per tile
-constexpr int BK = 64;   // fp16 elements per 128B swizzle atom row
-constexpr int ATOM_BYTES = 128 * BK * 2;  // 16 KiB: 128 rows x 64 fp16
-constexpr int NUM_THREADS = 192;
+constexpr int BN = 64;   // keys per tile
+constexpr int BK = 64;   // 16-bit elements per 128B swizzle atom row
+constexpr int Q_ATOM = BM * BK * 2;  // 16 KiB: 128 rows x 64 fp16
+constexpr int K_ATOM = BN * BK * 2;  // 8 KiB: 64 rows x 64 fp16
+constexpr int NUM_THREADS = 32 * CONSUMER_WARPS + 32;
 constexpr int MAX_KSTAGES = 8;
 constexpr int MAX_VSTAGES = 2;
-constexpr float RESCALE_THRESHOLD = 8.0f;  // log2 units (P stays <= 2^8)
 
 struct FwdParams {
   int B, Nq, Nk, Kd, Cv, Cvp;
   int kc_count;    // Kd / 64
-  int n_tiles;     // ceil(Nk / 128)
+  int n_tiles;     // ceil(Nk / 64)
   int q_resident;  // Q tile kept in smem for the whole CTA
   int ns_k, ns_v;
+  int v_stage;     // bytes per V stage
   float scale, scale_log2;
   float* out;   // [B, Cv, Nq]
   float* lse;   // [B, Nq] (natural log) or null
@@ -50,14 +51,19 @@ struct Barriers {
   uint64_t k_empty[MAX_KSTAGES];
   uint64_t v_full[MAX_VSTAGES];
   uint64_t v_empty[MAX_VSTAGES];
-  uint64_t s_full[2];
-  uint64_t s_empty[2];
-  uint64_t p_full;
-  uint64_t pv_done;
-  uint32_t tmem_base;
-  uint32_t pad;
 };
 
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
+// PVN: wgmma N of the P V product (tensor path) or 0; CV: value channels of the CUDA-core path or 0
+template <int PVN, int CV>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 corr_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
                 const __grid_constant__ CUtensorMap tm_v, const FwdParams p) {
@@ -72,57 +78,42 @@ corr_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   const int q0 = blockIdx.x * BM;
   const int bidx = blockIdx.y;
 
-  const uint32_t stage_bytes = p.q_resident ? ATOM_BYTES : 2 * ATOM_BYTES;
-  const uint32_t v_stage_bytes = static_cast<uint32_t>(p.Cvp) * 256u;  // 2 atoms of [Cvp x 64] fp16
+  const uint32_t stage_bytes = p.q_resident ? K_ATOM : Q_ATOM + K_ATOM;
   const uint32_t q_smem = smem0;
-  const uint32_t k_ring = q_smem + (p.q_resident ? p.kc_count * ATOM_BYTES : 0);
+  const uint32_t k_ring = q_smem + (p.q_resident ? p.kc_count * Q_ATOM : 0);
   const uint32_t v_ring = k_ring + p.ns_k * stage_bytes;
-  const uint32_t p_smem = v_ring + p.ns_v * v_stage_bytes;
-  const uint32_t bar_off = p_smem + 2 * ATOM_BYTES - smem0;
-  Barriers* bars = reinterpret_cast<Barriers*>(smem_gen + bar_off);
+  const uint32_t bar_off = v_ring + p.ns_v * p.v_stage - smem0;
+  Barriers* bars = reinterpret_cast<Barriers*>(smem_gen + ((bar_off + 7) & ~7u));
 
   if (tid == 0) {
     mbar_init(smem_u32(&bars->q_full), 1);
     for (int i = 0; i < p.ns_k; ++i) {
       mbar_init(smem_u32(&bars->k_full[i]), 1);
-      mbar_init(smem_u32(&bars->k_empty[i]), 1);
+      mbar_init(smem_u32(&bars->k_empty[i]), CONSUMER_WARPS);
     }
     for (int i = 0; i < p.ns_v; ++i) {
       mbar_init(smem_u32(&bars->v_full[i]), 1);
-      mbar_init(smem_u32(&bars->v_empty[i]), 1);
+      mbar_init(smem_u32(&bars->v_empty[i]), CONSUMER_WARPS);
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(smem_u32(&bars->s_full[i]), 1);
-      mbar_init(smem_u32(&bars->s_empty[i]), 128);
-    }
-    mbar_init(smem_u32(&bars->p_full), 128);
-    mbar_init(smem_u32(&bars->pv_done), 1);
     fence_mbar_init();
   }
-  if (warp == 4 && lane == 0) {
+  if (warp == CONSUMER_WARPS && lane == 0) {
     tma_prefetch_desc(&tm_q);
     tma_prefetch_desc(&tm_k);
     tma_prefetch_desc(&tm_v);
   }
-  if (warp == 5) {
-    tmem_alloc(smem_u32(&bars->tmem_base), 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = bars->tmem_base;
-  const uint32_t tmem_o = tmem + 256;  // S0: [0,128) S1: [128,256) O: [256, 256+Cvp)
   const int T = p.n_tiles;
 
-  if (warp == 4) {
+  if (warp == CONSUMER_WARPS) {
     // ------------------------------------------------------------ TMA producer
     if (lane == 0) {
       if (p.q_resident) {
-        mbar_expect_tx(smem_u32(&bars->q_full), p.kc_count * ATOM_BYTES);
+        mbar_expect_tx(smem_u32(&bars->q_full), p.kc_count * Q_ATOM);
         for (int kc = 0; kc < p.kc_count; ++kc)
-          tma_load_3d(q_smem + kc * ATOM_BYTES, &tm_q, smem_u32(&bars->q_full), kc * BK, q0, bidx);
+          tma_load_3d(q_smem + kc * Q_ATOM, &tm_q, smem_u32(&bars->q_full), kc * BK, q0, bidx);
       }
+      const uint32_t v_bytes = PVN ? static_cast<uint32_t>(p.Cvp) * BN * 2 : static_cast<uint32_t>(CV) * BN * 4;
       uint32_t ks = 0, kph = 0, vs = 0, vph = 0;
       for (int j = 0; j < T; ++j) {
         for (int kc = 0; kc < p.kc_count; ++kc) {
@@ -132,184 +123,163 @@ corr_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
           uint32_t dst = k_ring + ks * stage_bytes;
           if (!p.q_resident) {
             tma_load_3d(dst, &tm_q, full, kc * BK, q0, bidx);
-            dst += ATOM_BYTES;
+            dst += Q_ATOM;
           }
           tma_load_3d(dst, &tm_k, full, kc * BK, j * BN, bidx);
           if (++ks == static_cast<uint32_t>(p.ns_k)) { ks = 0; kph ^= 1; }
         }
         mbar_wait(smem_u32(&bars->v_empty[vs]), vph ^ 1);
         const uint32_t vfull = smem_u32(&bars->v_full[vs]);
-        mbar_expect_tx(vfull, v_stage_bytes);
-        const uint32_t vdst = v_ring + vs * v_stage_bytes;
-        tma_load_3d(vdst, &tm_v, vfull, j * BN, 0, bidx);
-        tma_load_3d(vdst + v_stage_bytes / 2, &tm_v, vfull, j * BN + BK, 0, bidx);
+        mbar_expect_tx(vfull, v_bytes);
+        tma_load_3d(v_ring + vs * p.v_stage, &tm_v, vfull, j * BN, 0, bidx);
         if (++vs == static_cast<uint32_t>(p.ns_v)) { vs = 0; vph ^= 1; }
       }
     }
     __syncwarp();
-  } else if (warp == 5) {
-    // -------------------------------------------------------------- MMA issuer
-    if (lane == 0) {
-      const uint32_t idesc_s = make_idesc_f16(BM, BN);
-      const uint32_t idesc_pv = make_idesc_f16(BM, p.Cvp);
-      uint32_t ks = 0, kph = 0, vs = 0, vph = 0;
-      if (p.q_resident) {
-        mbar_wait(smem_u32(&bars->q_full), 0);
-        tc_fence_after();
-      }
-      auto issue_s = [&](int t) {
-        const int b = t & 1;
-        if (t >= 2) {
-          mbar_wait(smem_u32(&bars->s_empty[b]), ((t >> 1) - 1) & 1);
-          tc_fence_after();
-        }
-        const uint32_t d_tmem = tmem + b * BN;
-        for (int kc = 0; kc < p.kc_count; ++kc) {
-          mbar_wait(smem_u32(&bars->k_full[ks]), kph);
-          tc_fence_after();
-          const uint32_t st = k_ring + ks * stage_bytes;
-          const uint32_t a_addr = p.q_resident ? (q_smem + kc * ATOM_BYTES) : st;
-          const uint32_t b_addr = p.q_resident ? st : (st + ATOM_BYTES);
+    return;
+  }
+
+  // ------------------------------------------------- softmax warpgroups (warps 0..7)
+  const int wg = tid >> 7, t = tid & 127;
+  const int r0 = 64 * wg + 16 * (t >> 5) + ((t & 31) >> 2);  // fragment rows r0 and r0 + 8
+  const int cq = 2 * (t & 3);                                 // fragment column offset
+  const float c2 = p.scale_log2;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  constexpr int ON = PVN ? PVN / 2 : 1;
+  float o[ON];
+  float oc[2][CV > 0 ? CV : 1];
 #pragma unroll
-          for (int s4 = 0; s4 < 4; ++s4) {
-            umma_f16(d_tmem, make_desc_k_sw128(a_addr + s4 * 32), make_desc_k_sw128(b_addr + s4 * 32), idesc_s,
-                     (kc | s4) != 0 ? 1u : 0u);
-          }
-          umma_commit(smem_u32(&bars->k_empty[ks]));
-          if (++ks == static_cast<uint32_t>(p.ns_k)) { ks = 0; kph ^= 1; }
-        }
-        umma_commit(smem_u32(&bars->s_full[b]));
-      };
-      issue_s(0);
-      for (int j = 0; j < T; ++j) {
-        if (j + 1 < T) issue_s(j + 1);
-        mbar_wait(smem_u32(&bars->p_full), j & 1);
-        mbar_wait(smem_u32(&bars->v_full[vs]), vph);
-        tc_fence_after();
-        const uint32_t vb = v_ring + vs * v_stage_bytes;
+  for (int i = 0; i < ON; ++i) o[i] = 0.f;
 #pragma unroll
-        for (int st = 0; st < 8; ++st) {
-          const uint32_t a_addr = p_smem + (st >> 2) * ATOM_BYTES + (st & 3) * 32;
-          const uint32_t b_addr = vb + (st >> 2) * (v_stage_bytes / 2) + (st & 3) * 32;
-          umma_f16(tmem_o, make_desc_k_sw128(a_addr), make_desc_k_sw128(b_addr), idesc_pv,
-                   (j | st) != 0 ? 1u : 0u);
-        }
-        umma_commit(smem_u32(&bars->v_empty[vs]));
-        umma_commit(smem_u32(&bars->pv_done));
-        if (++vs == static_cast<uint32_t>(p.ns_v)) { vs = 0; vph ^= 1; }
-      }
+  for (int r = 0; r < 2; ++r)
+#pragma unroll
+    for (int c = 0; c < (CV > 0 ? CV : 1); ++c) oc[r][c] = 0.f;
+
+  if (p.q_resident) mbar_wait(smem_u32(&bars->q_full), 0);
+  uint32_t ks = 0, kph = 0, vs = 0, vph = 0;
+  for (int j = 0; j < T; ++j) {
+    float s[BN / 2];
+    for (int kc = 0; kc < p.kc_count; ++kc) {
+      mbar_wait_quiet(smem_u32(&bars->k_full[ks]), kph);
+      const uint32_t st = k_ring + ks * stage_bytes;
+      const uint32_t a_addr = (p.q_resident ? (q_smem + kc * Q_ATOM) : st) + wg * 64 * 128;
+      const uint32_t b_addr = p.q_resident ? st : (st + Q_ATOM);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_ss<BN, false>(s, desc_advance_k16(make_desc_k_sw128(a_addr), k),
+                            desc_advance_k16(make_desc_k_sw128(b_addr), k), (kc | k) != 0 ? 1 : 0, 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(smem_u32(&bars->k_empty[ks]));
+      if (++ks == static_cast<uint32_t>(p.ns_k)) { ks = 0; kph ^= 1; }
     }
-    __syncwarp();
-  } else {
-    // ------------------------------------------------- softmax warps (0..3)
-    const int row = tid;  // TMEM lane == query row within the tile
-    const int q = q0 + row;
-    const uint32_t lane_sel = static_cast<uint32_t>(warp * 32) << 16;
-    const float c2 = p.scale_log2;
-    float m = -INFINITY, l = 0.f;
-    const uint32_t row_off = p_smem + row * 128;
-    const uint32_t sw = static_cast<uint32_t>(row & 7);
 
-    for (int j = 0; j < T; ++j) {
-      const int b = j & 1;
-      mbar_wait(smem_u32(&bars->s_full[b]), (j >> 1) & 1);
-      tc_fence_after();
-      float s[BN];
-#pragma unroll
-      for (int c = 0; c < 4; ++c)
-        tmem_ld32(tmem + lane_sel + b * BN + c * 32, reinterpret_cast<uint32_t*>(&s[c * 32]));
-      tmem_wait_ld();
-      tc_fence_before();
-      mbar_arrive(smem_u32(&bars->s_empty[b]));
-
-      if (p.corr != nullptr && q < p.Nq) {
-        float* dst = p.corr + (static_cast<size_t>(bidx) * p.Nq + q) * p.Nk + j * BN;
-        const int valid = p.Nk - j * BN;
-#pragma unroll
-        for (int c = 0; c < BN; ++c)
-          if (c < valid) dst[c] = s[c] * p.scale;
-      }
-      if (j == T - 1 && (p.Nk & (BN - 1)) != 0) {
-        const int valid = p.Nk - j * BN;
-#pragma unroll
-        for (int c = 0; c < BN; ++c)
-          if (c >= valid) s[c] = -INFINITY;
-      }
-      float tmax = s[0];
-#pragma unroll
-      for (int c = 1; c < BN; ++c) tmax = fmaxf(tmax, s[c]);
-      const float m_new = fmaxf(m, tmax);
-      if (j == 0) {
-        m = m_new;
-      } else {
-        const bool resc = (m_new - m) * c2 > RESCALE_THRESHOLD;
-        if (__any_sync(0xffffffffu, resc)) {
-          const float alpha = resc ? ex2((m - m_new) * c2) : 1.0f;
-          if (resc) m = m_new;
-          l *= alpha;
-          mbar_wait(smem_u32(&bars->pv_done), (j - 1) & 1);
-          tc_fence_after();
-          for (int cc = 0; cc < p.Cvp; cc += 16) {
-            uint32_t o[16];
-            tmem_ld16(tmem_o + lane_sel + cc, o);
-            tmem_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st16(tmem_o + lane_sel + cc, o);
-          }
-          tmem_wait_st();
-          tc_fence_before();
-        }
-      }
-      const float mc = m * c2;
-      float sum = 0.f;
-      uint32_t pk[BN / 2];
+    const int kbase = j * BN + cq;
+    if (p.corr != nullptr) {
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) {
-        const float p0 = ex2(fmaf(s[2 * i], c2, -mc));
-        const float p1 = ex2(fmaf(s[2 * i + 1], c2, -mc));
-        sum += p0 + p1;
-        pk[i] = pack_h2(p0, p1);
+        const int q = q0 + r0 + ((i >> 1) & 1) * 8, key = kbase + 8 * (i >> 2) + (i & 1);
+        if (q < p.Nq && key < p.Nk) p.corr[(static_cast<size_t>(bidx) * p.Nq + q) * p.Nk + key] = s[i] * p.scale;
       }
-      l += sum;
-      if (j > 0) mbar_wait(smem_u32(&bars->pv_done), (j - 1) & 1);  // P buffer free again
-#pragma unroll
-      for (int c = 0; c < 16; ++c) {
-        const uint32_t addr = row_off + (c >> 3) * ATOM_BYTES + (((c & 7) ^ sw) << 4);
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(pk[4 * c]), "r"(pk[4 * c + 1]),
-                     "r"(pk[4 * c + 2]), "r"(pk[4 * c + 3])
-                     : "memory");
-      }
-      fence_proxy_async_smem();
-      mbar_arrive(smem_u32(&bars->p_full));
     }
-
-    // epilogue: O / l -> out[b, c, q]
-    mbar_wait(smem_u32(&bars->pv_done), (T - 1) & 1);
-    tc_fence_after();
-    const float inv_l = 1.0f / l;
-    for (int cc = 0; cc < p.Cvp; cc += 16) {
-      uint32_t o[16];
-      tmem_ld16(tmem_o + lane_sel + cc, o);
-      tmem_wait_ld();
-      if (q < p.Nq) {
+    if (j == T - 1 && (p.Nk % BN) != 0) {
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const int c = cc + i;
-          if (c < p.Cv) p.out[(static_cast<size_t>(bidx) * p.Cv + c) * p.Nq + q] = __uint_as_float(o[i]) * inv_l;
+      for (int i = 0; i < BN / 2; ++i)
+        if (kbase + 8 * (i >> 2) + (i & 1) >= p.Nk) s[i] = -INFINITY;
+    }
+    float alpha[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      float tmax = -INFINITY;
+#pragma unroll
+      for (int jj = 0; jj < BN / 8; ++jj) tmax = fmaxf(tmax, fmaxf(s[4 * jj + 2 * r], s[4 * jj + 2 * r + 1]));
+      const float m_new = fmaxf(m[r], quad_max(tmax));  // finite: every tile has a valid key
+      alpha[r] = ex2((m[r] - m_new) * c2);                // exact online softmax; 0 on the first tile
+      m[r] = m_new;
+      l[r] *= alpha[r];
+    }
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) {
+      const int r = (i >> 1) & 1;
+      s[i] = ex2(fmaf(s[i], c2, -m[r] * c2));
+      l[r] += s[i];
+    }
+    mbar_wait_quiet(smem_u32(&bars->v_full[vs]), vph);
+    if constexpr (PVN > 0) {
+#pragma unroll
+      for (int i = 0; i < ON; ++i) o[i] *= alpha[(i >> 1) & 1];
+      const uint32_t vb = v_ring + vs * p.v_stage;
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < BN / 16; ++kk) {
+        uint32_t a[4];
+        a[0] = pack_h2(s[8 * kk + 0], s[8 * kk + 1]);
+        a[1] = pack_h2(s[8 * kk + 2], s[8 * kk + 3]);
+        a[2] = pack_h2(s[8 * kk + 4], s[8 * kk + 5]);
+        a[3] = pack_h2(s[8 * kk + 6], s[8 * kk + 7]);
+        wgmma_rs<PVN>(o, a, desc_advance_k16(make_desc_k_sw128(vb), kk), 1);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+    } else {
+      const float* vt = reinterpret_cast<const float*>(smem_gen + (v_ring - smem0) + vs * p.v_stage);
+#pragma unroll
+      for (int r = 0; r < 2; ++r)
+#pragma unroll
+        for (int c = 0; c < CV; ++c) oc[r][c] *= alpha[r];
+#pragma unroll
+      for (int jj = 0; jj < BN / 8; ++jj) {
+#pragma unroll
+        for (int c = 0; c < CV; ++c) {
+          const float2 v = *reinterpret_cast<const float2*>(vt + c * BN + 8 * jj + cq);
+#pragma unroll
+          for (int r = 0; r < 2; ++r) oc[r][c] = fmaf(s[4 * jj + 2 * r], v.x, fmaf(s[4 * jj + 2 * r + 1], v.y, oc[r][c]));
         }
       }
     }
-    if (p.lse != nullptr && q < p.Nq)
-      p.lse[static_cast<size_t>(bidx) * p.Nq + q] = (m * c2 + log2f(l)) * 0.6931471805599453f;
-    tc_fence_before();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(smem_u32(&bars->v_empty[vs]));
+    if (++vs == static_cast<uint32_t>(p.ns_v)) { vs = 0; vph ^= 1; }
   }
 
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 512);
+  // epilogue: O / l -> out[b, c, q]
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const float lt = quad_sum(l[r]);
+    const float inv_l = 1.0f / lt;
+    const int q = q0 + r0 + 8 * r;
+    if constexpr (PVN > 0) {
+      if (q < p.Nq) {
+#pragma unroll
+        for (int i = 0; i < ON; ++i) {
+          if (((i >> 1) & 1) != r) continue;
+          const int c = 8 * (i >> 2) + cq + (i & 1);
+          if (c < p.Cv) p.out[(static_cast<size_t>(bidx) * p.Cv + c) * p.Nq + q] = o[i] * inv_l;
+        }
+      }
+    } else {
+#pragma unroll
+      for (int c = 0; c < CV; ++c) {
+        const float v = quad_sum(oc[r][c]);
+        if (q < p.Nq && (t & 3) == c) p.out[(static_cast<size_t>(bidx) * p.Cv + c) * p.Nq + q] = v * inv_l;
+      }
+    }
+    if (p.lse != nullptr && q < p.Nq && (t & 3) == 0)
+      p.lse[static_cast<size_t>(bidx) * p.Nq + q] = (m[r] * c2 + log2f(lt)) * 0.6931471805599453f;
   }
+}
+
+template <int PVN, int CV>
+int launch_fwd(const CUtensorMap& tm_q, const CUtensorMap& tm_k, const CUtensorMap& tm_v, const FwdParams& p,
+               int smem_bytes, cudaStream_t stream) {
+  COCOS_CUDA_CHECK(
+      cudaFuncSetAttribute(corr_fwd_kernel<PVN, CV>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+  dim3 grid((p.Nq + BM - 1) / BM, p.B);
+  corr_fwd_kernel<PVN, CV><<<grid, NUM_THREADS, smem_bytes, stream>>>(tm_q, tm_k, tm_v, p);
+  COCOS_CUDA_CHECK(cudaGetLastError());
+  return 0;
 }
 
 }  // namespace
@@ -325,37 +295,21 @@ int corr_warp_fwd_launch(const void* q, const void* k, const void* vt, const flo
     set_error("corr_warp_fwd: Kd=%d must be a positive multiple of 64 (pad in the pack kernel)", Kd);
     return -1;
   }
-  static const int variant = [] {
-    // default: best kernel that applies; COCOS_K1_VARIANT=1..4 caps the choice (A/B timing)
-    const char* e = getenv("COCOS_K1_VARIANT");
-    return e ? atoi(e) : 4;
-  }();
-  if (variant >= 4 && v32 != nullptr && corr == nullptr && Cv >= 1 && Cv <= 4) {
-    const int rc4 = corr_warp_fwd4_launch(q, k, v32, out, lse, B, Nq, Nk, Kd, Cv, scale, stream);
-    if (rc4 != 1) return rc4;
-  }
-  if (vt == nullptr) {
-    set_error("corr_warp_fwd: packed fp16 values (vt) are required for this shape (Cv=%d)", Cv);
-    return -1;
-  }
-  if (Cv <= 0 || Cvp < Cv || (Cvp % 16) != 0 || Cvp > 256) {
-    set_error("corr_warp_fwd: need 0 < Cv <= Cvp <= 256, Cvp %% 16 == 0 (Cv=%d Cvp=%d)", Cv, Cvp);
-    return -1;
-  }
-  if (Nkp < Nk || (Nkp % 8) != 0) {
-    set_error("corr_warp_fwd: V row pitch Nkp=%d must be >= Nk=%d and a multiple of 8", Nkp, Nk);
-    return -1;
-  }
-  {
-    // 256-key tiles (v3) when Cvp <= 64, else the two-warpgroup 128-key pipeline (v2), else the
-    // single-warpgroup kernel below
-    if (variant >= 3 && corr == nullptr && Cvp <= 64) {
-      const int rc3 = corr_warp_fwd3_launch(q, k, vt, out, lse, B, Nq, Nk, Kd, Cv, Cvp, Nkp, scale, stream);
-      if (rc3 != 1) return rc3;
+  // Cv <= 4 with fp32 values: P V on the CUDA cores (no fp16 rounding of P); otherwise the tensor-core P V
+  const bool cuda_pv = v32 != nullptr && corr == nullptr && Cv >= 1 && Cv <= 4 && (Nk % 4) == 0 &&
+                       (reinterpret_cast<uintptr_t>(v32) & 15) == 0;
+  if (!cuda_pv) {
+    if (vt == nullptr) {
+      set_error("corr_warp_fwd: packed fp16 values (vt) are required for this shape (Cv=%d)", Cv);
+      return -1;
     }
-    if (variant >= 2 && corr == nullptr && Cvp <= 128) {
-      const int rc2 = corr_warp_fwd2_launch(q, k, vt, out, lse, B, Nq, Nk, Kd, Cv, Cvp, Nkp, scale, stream);
-      if (rc2 != 1) return rc2;
+    if (Cv <= 0 || Cvp < Cv || (Cvp % 16) != 0 || Cvp > 256) {
+      set_error("corr_warp_fwd: need 0 < Cv <= Cvp <= 256, Cvp %% 16 == 0 (Cv=%d Cvp=%d)", Cv, Cvp);
+      return -1;
+    }
+    if (Nkp < Nk || (Nkp % 8) != 0) {
+      set_error("corr_warp_fwd: V row pitch Nkp=%d must be >= Nk=%d and a multiple of 8", Nkp, Nk);
+      return -1;
     }
   }
   FwdParams p;
@@ -365,40 +319,43 @@ int corr_warp_fwd_launch(const void* q, const void* k, const void* vt, const flo
   p.scale = scale;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.out = out; p.lse = lse; p.corr = corr;
+  const int pvn = cuda_pv ? 0 : (Cvp <= 64 ? 64 : Cvp <= 128 ? 128 : 256);
+  // a V stage holds PVN rows of 64 keys (the wgmma reads PVN >= Cvp rows) or Cv fp32 rows of 64 keys
+  p.v_stage = cuda_pv ? 1024 : pvn * BN * 2;
 
-  // shared memory plan (<= 227 KiB): [Q] [K ring] [V ring] [P] [barriers]
+  // shared memory plan (<= 227 KiB): [Q] [K ring] [V ring] [barriers]
   const int budget = 227 * 1024 - 1024 /*alignment slack*/ - 512 /*barriers*/;
-  const int p_bytes = 2 * ATOM_BYTES;
-  const int v_stage = Cvp * 256;
   p.q_resident = (Kd <= 256) ? 1 : 0;
-  const int q_bytes = p.q_resident ? p.kc_count * ATOM_BYTES : 0;
-  const int stage = p.q_resident ? ATOM_BYTES : 2 * ATOM_BYTES;
+  const int q_bytes = p.q_resident ? p.kc_count * Q_ATOM : 0;
+  const int stage = p.q_resident ? K_ATOM : Q_ATOM + K_ATOM;
   p.ns_v = 2;
-  int rem = budget - p_bytes - q_bytes - p.ns_v * v_stage;
-  if (rem / stage < 3) {
-    p.ns_v = 1;
-    rem = budget - p_bytes - q_bytes - v_stage;
-  }
-  p.ns_k = rem / stage;
+  p.ns_k = (budget - q_bytes - p.ns_v * p.v_stage) / stage;
   if (p.ns_k > MAX_KSTAGES) p.ns_k = MAX_KSTAGES;
   if (p.ns_k < 2) {
     set_error("corr_warp_fwd: shared memory plan failed (Kd=%d Cvp=%d)", Kd, Cvp);
     return -1;
   }
-  const int smem_bytes = 1024 + q_bytes + p.ns_k * stage + p.ns_v * v_stage + p_bytes + 512;
+  const int smem_bytes = 1024 + q_bytes + p.ns_k * stage + p.ns_v * p.v_stage + 512;
 
   CUtensorMap tm_q, tm_k, tm_v;
   int rc;
   if ((rc = make_tmap_f16_3d(&tm_q, q, Kd, Nq, B, (uint64_t)Kd * 2, (uint64_t)Nq * Kd * 2, BK, BM, 1))) return rc;
   if ((rc = make_tmap_f16_3d(&tm_k, k, Kd, Nk, B, (uint64_t)Kd * 2, (uint64_t)Nk * Kd * 2, BK, BN, 1))) return rc;
+  if (cuda_pv) {
+    if ((rc = make_tmap_f32_3d_plain(&tm_v, v32, Nk, Cv, B, (uint64_t)Nk * 4, (uint64_t)Cv * Nk * 4, BN, Cv, 1)))
+      return rc;
+    switch (Cv) {
+      case 1: return launch_fwd<0, 1>(tm_q, tm_k, tm_v, p, smem_bytes, stream);
+      case 2: return launch_fwd<0, 2>(tm_q, tm_k, tm_v, p, smem_bytes, stream);
+      case 3: return launch_fwd<0, 3>(tm_q, tm_k, tm_v, p, smem_bytes, stream);
+      default: return launch_fwd<0, 4>(tm_q, tm_k, tm_v, p, smem_bytes, stream);
+    }
+  }
   if ((rc = make_tmap_f16_3d(&tm_v, vt, Nk, Cvp, B, (uint64_t)Nkp * 2, (uint64_t)Cvp * Nkp * 2, BK, Cvp, 1)))
     return rc;
-
-  COCOS_CUDA_CHECK(cudaFuncSetAttribute(corr_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-  dim3 grid((Nq + BM - 1) / BM, B);
-  corr_fwd_kernel<<<grid, NUM_THREADS, smem_bytes, stream>>>(tm_q, tm_k, tm_v, p);
-  COCOS_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  if (pvn == 64) return launch_fwd<64, 0>(tm_q, tm_k, tm_v, p, smem_bytes, stream);
+  if (pvn == 128) return launch_fwd<128, 0>(tm_q, tm_k, tm_v, p, smem_bytes, stream);
+  return launch_fwd<256, 0>(tm_q, tm_k, tm_v, p, smem_bytes, stream);
 }
 
 }  // namespace cocos

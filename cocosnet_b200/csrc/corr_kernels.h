@@ -7,22 +7,10 @@
 
 namespace cocos {
 
-// v32 (optional): the values as fp32 [B, Cv, Nk]; with Cv <= 4 the CUDA-core-PV kernel (corr_fwd4.cu) is used
+// v32 (optional): the values as fp32 [B, Cv, Nk]; with Cv <= 4 the P V product runs on the CUDA cores in fp32
 int corr_warp_fwd_launch(const void* q, const void* k, const void* vt, const float* v32, float* out, float* lse,
                          float* corr, int B, int Nq, int Nk, int Kd, int Cv, int Cvp, int Nkp, float scale,
                          cudaStream_t stream);
-
-// Cv <= 4: P V on the CUDA cores inside the exp loop, S double buffered at N=256; returns 1 if it does not apply
-int corr_warp_fwd4_launch(const void* q, const void* k, const float* v, float* out, float* lse, int B, int Nq, int Nk,
-                          int Kd, int Cv, float scale, cudaStream_t stream);
-
-// two-softmax-warpgroup variant (Cvp <= 128, no corr dump); returns 1 if it does not apply
-int corr_warp_fwd2_launch(const void* q, const void* k, const void* vt, float* out, float* lse, int B, int Nq,
-                          int Nk, int Kd, int Cv, int Cvp, int Nkp, float scale, cudaStream_t stream);
-
-// 256-key S tiles (UMMA N=256), P in tensor memory (Cvp <= 64); returns 1 if it does not apply
-int corr_warp_fwd3_launch(const void* q, const void* k, const void* vt, float* out, float* lse, int B, int Nq,
-                          int Nk, int Kd, int Cv, int Cvp, int Nkp, float scale, cudaStream_t stream);
 
 // C[b] (MxN fp32, row-major, ldc) = alpha * A[b] (MxK fp16, K contiguous) * B[b]^T (NxK fp16) (+ C if accumulate)
 int gemm_f16_launch(const void* a, const void* b, float* c, int batch, int M, int N, int K, int lda, int ldb,
@@ -41,7 +29,8 @@ int pack_v_f16_launch(const float* src, void* dst, int B, int Cv, int Nk, int Cv
 int cast_pitch_launch(const float* src, void* dst, long long rows, int Win, int Wout, int Wp, int nshift, int off,
                       int bf16, cudaStream_t stream);
 int conv_wgrad_launch(const void* dy, const void* x, float* ws, int B, int H, int W, int Hin, int Win, int Cout, int Cin,
-                      int KS, int off, int a_bf16, int b_bf16, cudaStream_t stream);
+                      int KS, int off, int a_bf16, int b_bf16, float* ws_part, long long* ws_floats,
+                      cudaStream_t stream);
 int conv_fwd_launch(const void* x, const void* wt, const float* bias, float* y, int B, int H, int W, int Hin, int Win,
                     int Cp, int Cout, int KS, int off, int bf16, cudaStream_t stream);
 
@@ -70,7 +59,7 @@ namespace cocos {
 // 16-bit NHWC pipeline (tapconv.cu, tapwgrad.cu, ew_nhwc.cu)
 int tapconv_launch(const cocos_tapconv_desc* d, cudaStream_t stream);
 void tapconv_tile_shape(int B, int H, int W, int* TB, int* TH, int* TW);
-int tapwgrad_launch(const cocos_tapwgrad_desc* d, cudaStream_t stream);
+int tapwgrad_launch(const cocos_tapwgrad_desc* d, long long* need_out, cudaStream_t stream);
 int spade_mod_nhwc_fwd_launch(const void* x, int x_kind, int x_Cs, const void* gb, int gb_kind, int gb_Cs, void* y,
                               int y_Cs, int y_lo_off, float* mean, float* rstd, int B, int C, int H, int W, int pad,
                               float slope, float eps, cudaStream_t stream);
@@ -85,7 +74,8 @@ int spade_mod_nhwc_bwd_launch(const void* dy, int dy_Cs, const void* x, int x_ki
                               int gb_kind, int gb_Cs, int gb_W, const float* mean, const float* rstd, void* dx, int dx_Cs,
                               int dx_acc, void* dgb, int dgb_Cs, int B, int C, int H, int W, int pad, float slope,
                               cudaStream_t stream);
-int in_stats_nhwc_launch(const void* x, int kind, int Cs, int B, int C, int HW, float* stats, cudaStream_t stream);
+int in_stats_nhwc_launch(const void* x, int kind, int Cs, int B, int C, int HW, float* stats, float* ws,
+                         long long* ws_floats, cudaStream_t stream);
 int inst_act_nhwc_fwd_launch(const void* x, int x_kind, int x_Cs, const float* stats, const void* res, int res_kind,
                              int res_Cs, const float* slope_ptr, float slope, void* y, int y_kind, int y_Cs,
                              int y_lo_off, int y_pad, void* y2, int y2_Cs, int B, int C, int H, int W, float eps,
@@ -95,13 +85,13 @@ int inst_act_nhwc_bwd_launch(const void* dy, int dy_Cs, int dy_pad, const void* 
                              const float* slope_ptr, float slope, float* bstats, float* dslope, void* dx, int dx_Cs,
                              int dx_acc, void* dres, int dres_Cs, int dres_acc, int B, int C, int H, int W, float eps,
                              const void* gb, int gb_kind, int gb_Cs, void* dgb, int dgb_Cs, int batch_stats,
-                             int const_stats, int phase, cudaStream_t stream);
+                             int const_stats, int phase, float* ws, long long* ws_floats, cudaStream_t stream);
 int act_bwd_nhwc_launch(const void* dy, int dy_Cs, const void* y, int y_kind, int y_Cs, int pad, void* dz, int dz_Cs,
                         int B, int C, int H, int W, int act, float slope, cudaStream_t stream);
 int nhwc_pack_launch(const float* src, void* dst, int kind, int B, int C, int Cs, int lo_off, int c_lo, int c_span,
                      int Hs, int Ws, int H, int W, int f, int pad, cudaStream_t stream);
 int pair_loss_nhwc_fwd_launch(const void* x, int x_Cs, const void* y, int y_Cs, const float* w, int B, long long HW, int C,
-                              float scale, int mode, float* out, cudaStream_t stream);
+                              float scale, int mode, float* out, float* ws, long long* ws_floats, cudaStream_t stream);
 int pair_loss_nhwc_bwd_launch(const void* x, int x_Cs, const void* y, int y_Cs, const float* w, int B, long long HW, int C,
                               float scale, int mode, const float* g, void* dx, int dx_Cs, int acc, cudaStream_t stream);
 int cast_op_bf16_launch(const void* src, int src_Cs, int lo_off, void* dst, int dst_Cs, long long npix,
@@ -111,7 +101,8 @@ int maxpool2_nhwc_bwd_launch(const void* dy, const void* x, void* dx, int B, int
                              cudaStream_t stream);
 int nhwc_unpack_launch(const void* src, int kind, int Cs, int c_lo, int C, int B, int H, int W, int pad, float* dst,
                        int Cd, int cd_lo, int Hd, int Wd, int f, int acc, cudaStream_t stream);
-int colsum_nhwc_launch(const void* x, int kind, int Cs, int C, long long rows, float* out, cudaStream_t stream);
+int colsum_nhwc_launch(const void* x, int kind, int Cs, int C, long long rows, float* out, float* ws,
+                       long long* ws_floats, cudaStream_t stream);
 int pack_w_launch(const float* w, int Cout, int Cin, int KS, void* dst, int rows, int rows_alloc, int Kc, int ngroups,
                   const signed char* r, const signed char* s, const signed char* term, int transposed, int bf16,
                   cudaStream_t stream);

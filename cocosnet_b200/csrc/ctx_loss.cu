@@ -1,5 +1,5 @@
 // Row kernels of the contextual loss (reference models/networks/ContextualLoss.py:93-137) on the correlation matrix
-// S = Xhat^T Yhat [B, N, N] (fp32, produced by the tcgen05 GEMM cocos_gemm_f16; N <= 1024 positions of a VGG map):
+// S = Xhat^T Yhat [B, N, N] (fp32, produced by the wgmma GEMM cocos_gemm_f16; N <= 1024 positions of a VGG map):
 //   d = 1 - S,  m_i = min_j d_ij,  w_ij = exp((1 - d_ij / (m_i + 1e-3)) / h),  A_ij = w_ij / sum_j w_ij,
 //   CX_i = max_j A_ij = 1 / sum_j q_ij,  q_ij = exp(-a_i (d_ij - m_i)),  a_i = 1 / (h (m_i + 1e-3))
 // (w is decreasing in d, so the row maximum sits at the row minimum of d).  The reference materialises d, d_norm, w,

@@ -1,5 +1,5 @@
 // HBM-bound elementwise / normalisation kernels of the 16-bit NHWC pipeline (everything between two tap
-// convolutions), sm_100a.  Tensor "kinds": 1 = fp16, 2 = bf16, 3 = fp32; activations NHWC [B, H, W, Cs] with channel
+// convolutions), sm_90a.  Tensor "kinds": 1 = fp16, 2 = bf16, 3 = fp32; activations NHWC [B, H, W, Cs] with channel
 // stride Cs >= C; gradients bf16.  `op` tensors (the A operand of the next convolution) are fp16, optionally carry
 // a 1-pixel reflection halo ([B, H+2, W+2, Cs]) and optionally a second fp16 term lo = x - fp16(x) at channel
 // offset lo_off (2-term split operands of the correspondence path).
@@ -271,7 +271,7 @@ __device__ __forceinline__ Coef4 load_coef4(const float* __restrict__ stats, int
   return k;
 }
 
-// stats[b][c] = {sum, sumsq} over the H*W pixels; partial sums land with atomics (stats zeroed by the launcher).
+// part[chunk][b][c] = {sum, sumsq} over the chunk's pixels (blockIdx.x = chunk); ordered_sum() adds the chunks.
 __global__ void __launch_bounds__(256)
 in_stats_nhwc_kernel(const void* __restrict__ x, int kind, int Cs, int C, int HW, int pix_per_block,
                      float* __restrict__ stats) {
@@ -306,8 +306,9 @@ in_stats_nhwc_kernel(const void* __restrict__ x, int kind, int Cs, int C, int HW
         bq += red[k][threadIdx.x][4 + j];
       }
       if (c + j < C) {
-        atomicAdd(stats + (static_cast<size_t>(b) * C + c + j) * 2, a);
-        atomicAdd(stats + (static_cast<size_t>(b) * C + c + j) * 2 + 1, bq);
+        float* dst = stats + (static_cast<size_t>(blockIdx.x) * gridDim.z * C + static_cast<size_t>(b) * C + c + j) * 2;
+        dst[0] = a;
+        dst[1] = bq;
       }
     }
   }
@@ -432,7 +433,7 @@ __device__ __forceinline__ void inst_bwd_dz(const InstBwd& p, const Coef4& k, in
   }
 }
 
-// pass 1: bstats += {sum dz, sum dz*z}, dslope += sum dy*u*[u<=0]
+// pass 1: per-block partials of {sum dz, sum dz*z} (bstats) and of sum dy*u*[u<=0] (dslope)
 template <int MODE>
 __global__ void __launch_bounds__(256) inst_act_nhwc_bwd_stats_kernel(const InstBwd p, int pix_per_block) {
   __shared__ float red[8][32][8];
@@ -478,9 +479,11 @@ __global__ void __launch_bounds__(256) inst_act_nhwc_bwd_stats_kernel(const Inst
           bq += red[k][threadIdx.x][4 + j];
         }
         if (c + j < p.C) {
-          const size_t bo = (static_cast<size_t>(p.batch_stats ? 0 : b) * p.C + c + j) * 2;
-          atomicAdd(p.bstats + bo, a);
-          atomicAdd(p.bstats + bo + 1, bq);
+          // partial of (chunk, b): part[(chunk * B + b) * 2C + 2c] -- ordered_sum() adds the chunks (and, for batch
+          // statistics, the images) in a fixed order
+          float* dst = p.bstats + (static_cast<size_t>(blockIdx.x) * p.B + b) * 2 * p.C + 2 * (c + j);
+          dst[0] = a;
+          dst[1] = bq;
         }
       }
     }
@@ -488,7 +491,7 @@ __global__ void __launch_bounds__(256) inst_act_nhwc_bwd_stats_kernel(const Inst
       float t = 0.f;
       for (int k = 0; k < 8; ++k)
         for (int xx = 0; xx < static_cast<int>(blockDim.x); ++xx) t += red_s[k][xx];
-      atomicAdd(p.dslope, t);
+      p.dslope[blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z)] = t;  // one partial per block
     }
   }
 }
@@ -571,7 +574,7 @@ act_bwd_nhwc_kernel(const void* __restrict__ dy, int dy_Cs, const void* __restri
 // out[0] += scale * sum_b w[b] * sum_{pixels, c < C} |x - y|  (mode 0: criterionFeat / weighted_l1_loss,
 // pix2pix_model.py:240,253; util/util.py:36-40) or (x - y)^2 (mode 1: the perceptual MSE, pix2pix_model.py:256) over two
 // fp16 NHWC feature tensors -- the discriminator / VGG19 features never leave the 16-bit NHWC pipeline for their loss.
-// One block = 8 pixel lanes x 32 threads x 8 channels; block reduction, one atomic per block.
+// One block = 8 pixel lanes x 32 threads x 8 channels; block reduction, one partial per block (added in block order by ordered_sum).
 __global__ void __launch_bounds__(256)
 pair_loss_nhwc_fwd_kernel(const uint16_t* __restrict__ x, int x_Cs, const uint16_t* __restrict__ y, int y_Cs,
                           const float* __restrict__ w, int B, long long HW, int C8, float scale, int mode,
@@ -604,7 +607,7 @@ pair_loss_nhwc_fwd_kernel(const uint16_t* __restrict__ x, int x_Cs, const uint16
     float t = 0.f;
 #pragma unroll
     for (int k = 0; k < 8; ++k) t += red[k];
-    atomicAdd(out, t * scale);
+    out[blockIdx.x] = t * scale;  // one partial per block
   }
 }
 
@@ -646,9 +649,9 @@ pair_loss_nhwc_bwd_kernel(const uint16_t* __restrict__ x, int x_Cs, const uint16
 
 // ----------------------------------------------------------------------------------------------- fp16 -> bf16 operand
 // The backward-weights GEMM multiplies dY (bf16: gradients need the fp32 exponent range) with the activation X the
-// forward saved (fp16 [hi | lo]); tcgen05 cannot mix fp16 x bf16 operands, and converting X inside the GEMM kernel
-// costs a third of its throughput (profiles/r02_tapconv_bf16x.txt).  So X is converted here, once per tensor, in an
-// HBM-bound pass: dst[pix][c] = bf16(hi + lo), 8 channels (16 bytes) per thread, halo pixels included.
+// forward saved (fp16 [hi | lo]); wgmma cannot mix fp16 x bf16 operands, and converting X inside the GEMM kernel
+// repeats the conversion for every output-channel tile.  So X is converted here, once per tensor, in an HBM-bound
+// pass: dst[pix][c] = bf16(hi + lo), 8 channels (16 bytes) per thread, halo pixels included.
 __global__ void __launch_bounds__(256)
 cast_op_bf16_kernel(const uint16_t* __restrict__ src, int src_Cs, int lo_off, uint16_t* __restrict__ dst, int dst_Cs,
                     long long npix) {
@@ -870,7 +873,7 @@ nhwc_unpack16_kernel(const uint16_t* __restrict__ src, int bf16, int Cs, int c_l
   }
 }
 
-// db[c] += sum over rows of a 16-bit / fp32 [rows, Cs] matrix (out zeroed by the launcher); grid (row chunks, C/128)
+// part[chunk][c] = sum over the chunk's rows of a 16-bit / fp32 [rows, Cs] matrix; grid (row chunks, C/128)
 __global__ void __launch_bounds__(256)
 colsum_nhwc_kernel(const void* __restrict__ x, int kind, int Cs, int C, long long rows, int rows_per_block,
                    float* __restrict__ out) {
@@ -895,7 +898,7 @@ colsum_nhwc_kernel(const void* __restrict__ x, int kind, int Cs, int C, long lon
       float a = 0.f;
 #pragma unroll
       for (int k = 0; k < 8; ++k) a += red[k][threadIdx.x][j];
-      if (c + j < C) atomicAdd(out + c + j, a);
+      if (c + j < C) out[static_cast<size_t>(blockIdx.x) * C + c + j] = a;
     }
   }
 }
@@ -999,7 +1002,7 @@ static void stats_grid(int HW, int C, int B, dim3* grid, dim3* block, int* ppb) 
   const int c4 = (C + 3) / 4;
   const int cg = (c4 + 31) / 32;
   const int tx = (c4 + cg - 1) / cg;
-  int chunks = (8 * 148 + cg * B - 1) / (cg * B);
+  int chunks = (8 * num_sms() + cg * B - 1) / (cg * B);
   const int max_chunks = (HW + 63) / 64;
   if (chunks > max_chunks) chunks = max_chunks;
   if (chunks < 1) chunks = 1;
@@ -1008,18 +1011,22 @@ static void stats_grid(int HW, int C, int B, dim3* grid, dim3* block, int* ppb) 
   *block = dim3(tx, 8);
 }
 
-int in_stats_nhwc_launch(const void* x, int kind, int Cs, int B, int C, int HW, float* stats, cudaStream_t stream) {
+int in_stats_nhwc_launch(const void* x, int kind, int Cs, int B, int C, int HW, float* stats, float* ws,
+                         long long* ws_floats, cudaStream_t stream) {
   if (B <= 0 || C <= 0 || (C % 4) || (Cs % 4) || HW <= 0 || kind < 1 || kind > 3) {
     set_error("in_stats_nhwc: bad arguments (B=%d C=%d HW=%d)", B, C, HW);
     return -1;
   }
-  COCOS_CUDA_CHECK(cudaMemsetAsync(stats, 0, sizeof(float) * 2 * B * C, stream));
   dim3 grid, block;
   int ppb;
   stats_grid(HW, C, B, &grid, &block, &ppb);
-  in_stats_nhwc_kernel<<<grid, block, 0, stream>>>(x, kind, Cs, C, HW, ppb, stats);
+  const long long n = 2ll * B * C;
+  const int wc = workspace_check(ws, ws_floats, grid.x * n, "in_stats_nhwc");
+  if (wc) return wc < 0 ? -1 : 0;
+  float* part = ws;
+  in_stats_nhwc_kernel<<<grid, block, 0, stream>>>(x, kind, Cs, C, HW, ppb, part);
   COCOS_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return ordered_sum(part, grid.x, n, stats, 0, stream);
 }
 
 int inst_act_nhwc_fwd_launch(const void* x, int x_kind, int x_Cs, const float* stats, const void* res, int res_kind,
@@ -1048,7 +1055,7 @@ int inst_act_nhwc_bwd_launch(const void* dy, int dy_Cs, int dy_pad, const void* 
                              const float* slope_ptr, float slope, float* bstats, float* dslope, void* dx, int dx_Cs,
                              int dx_acc, void* dres, int dres_Cs, int dres_acc, int B, int C, int H, int W, float eps,
                              const void* gb, int gb_kind, int gb_Cs, void* dgb, int dgb_Cs, int batch_stats,
-                             int const_stats, int phase, cudaStream_t stream) {
+                             int const_stats, int phase, float* ws, long long* ws_floats, cudaStream_t stream) {
   if (B <= 0 || C <= 0 || (C % 4) || (dy_Cs % 4) || (x_Cs % 4) || (dx_Cs % 4) || H <= dy_pad || W <= dy_pad ||
       dy_pad < 0 || dy_pad > 1 || x_kind < 1 || x_kind > 3 || (res && (res_kind < 1 || res_kind > 3 || (res_Cs % 4))) ||
       (dy2 && (dy2_Cs % 4)) || (dres && (dres_Cs % 4)) || !bstats || phase < 0 || phase > 2 ||
@@ -1067,23 +1074,45 @@ int inst_act_nhwc_bwd_launch(const void* dy, int dy_Cs, int dy_pad, const void* 
   int mode = -1;
   if (!gb && (x_kind == 1 || x_kind == 3) && (!res || res_kind == x_kind))
     mode = (x_kind == 3 ? 1 : 0) | (res ? 2 : 0) | (dy_pad ? 4 : 0) | (dy2 ? 8 : 0);
-#define COCOS_INST_BWD(M)                                                                      \
-  case M:                                                                                      \
-    if (phase != 2) inst_act_nhwc_bwd_stats_kernel<M><<<grid, block, 0, stream>>>(p, ppb);     \
-    if (phase != 1) inst_act_nhwc_bwd_apply_kernel<M><<<grid, block, 0, stream>>>(p, ppb);     \
-    break;
-  if (phase != 2)
-    COCOS_CUDA_CHECK(cudaMemsetAsync(bstats, 0, sizeof(float) * 2 * (batch_stats ? 1 : B) * C, stream));
-  switch (mode) {
-    COCOS_INST_BWD(0) COCOS_INST_BWD(1) COCOS_INST_BWD(2) COCOS_INST_BWD(3) COCOS_INST_BWD(4) COCOS_INST_BWD(5)
-    COCOS_INST_BWD(6) COCOS_INST_BWD(7) COCOS_INST_BWD(8) COCOS_INST_BWD(9) COCOS_INST_BWD(10) COCOS_INST_BWD(11)
-    COCOS_INST_BWD(12) COCOS_INST_BWD(13) COCOS_INST_BWD(14) COCOS_INST_BWD(15)
-    default:
-      if (phase != 2) inst_act_nhwc_bwd_stats_kernel<-1><<<grid, block, 0, stream>>>(p, ppb);
-      if (phase != 1) inst_act_nhwc_bwd_apply_kernel<-1><<<grid, block, 0, stream>>>(p, ppb);
-  }
+  // the statistics kernel writes per-block partials into the workspace: [chunk][b][2C] for bstats, then one per block
+  // for dslope; ordered_sum() reduces them in a fixed order before the apply kernel reads bstats
+  const long long nb = 2ll * B * C, nblocks = static_cast<long long>(grid.x) * grid.y * grid.z;
+  const int wc = workspace_check(ws, ws_floats, phase != 2 ? grid.x * nb + nblocks : 0, "inst_act_nhwc_bwd");
+  if (wc) return wc < 0 ? -1 : 0;
+  if (phase != 2) {
+    float* part = ws;
+    InstBwd ps = p;
+    ps.bstats = part;
+    ps.dslope = dslope ? part + grid.x * nb : nullptr;
+#define COCOS_INST_BWD(M) \
+  case M: inst_act_nhwc_bwd_stats_kernel<M><<<grid, block, 0, stream>>>(ps, ppb); break;
+    switch (mode) {
+      COCOS_INST_BWD(0) COCOS_INST_BWD(1) COCOS_INST_BWD(2) COCOS_INST_BWD(3) COCOS_INST_BWD(4) COCOS_INST_BWD(5)
+      COCOS_INST_BWD(6) COCOS_INST_BWD(7) COCOS_INST_BWD(8) COCOS_INST_BWD(9) COCOS_INST_BWD(10) COCOS_INST_BWD(11)
+      COCOS_INST_BWD(12) COCOS_INST_BWD(13) COCOS_INST_BWD(14) COCOS_INST_BWD(15)
+      default: inst_act_nhwc_bwd_stats_kernel<-1><<<grid, block, 0, stream>>>(ps, ppb);
+    }
 #undef COCOS_INST_BWD
-  COCOS_CUDA_CHECK(cudaGetLastError());
+    COCOS_CUDA_CHECK(cudaGetLastError());
+    int rc;
+    // batch statistics: [chunk * B + b][2C] summed over chunks and images; per image: [chunk][2BC] over chunks
+    if ((rc = batch_stats ? ordered_sum(part, grid.x * B, 2ll * C, bstats, 0, stream)
+                          : ordered_sum(part, grid.x, nb, bstats, 0, stream)))
+      return rc;
+    if (dslope && (rc = ordered_sum(part + grid.x * nb, static_cast<int>(nblocks), 1, dslope, 1, stream))) return rc;
+  }
+  if (phase != 1) {
+#define COCOS_INST_BWD(M) \
+  case M: inst_act_nhwc_bwd_apply_kernel<M><<<grid, block, 0, stream>>>(p, ppb); break;
+    switch (mode) {
+      COCOS_INST_BWD(0) COCOS_INST_BWD(1) COCOS_INST_BWD(2) COCOS_INST_BWD(3) COCOS_INST_BWD(4) COCOS_INST_BWD(5)
+      COCOS_INST_BWD(6) COCOS_INST_BWD(7) COCOS_INST_BWD(8) COCOS_INST_BWD(9) COCOS_INST_BWD(10) COCOS_INST_BWD(11)
+      COCOS_INST_BWD(12) COCOS_INST_BWD(13) COCOS_INST_BWD(14) COCOS_INST_BWD(15)
+      default: inst_act_nhwc_bwd_apply_kernel<-1><<<grid, block, 0, stream>>>(p, ppb);
+    }
+#undef COCOS_INST_BWD
+    COCOS_CUDA_CHECK(cudaGetLastError());
+  }
   return 0;
 }
 
@@ -1144,18 +1173,22 @@ int nhwc_unpack_launch(const void* src, int kind, int Cs, int c_lo, int C, int B
 }
 
 int pair_loss_nhwc_fwd_launch(const void* x, int x_Cs, const void* y, int y_Cs, const float* w, int B, long long HW, int C,
-                              float scale, int mode, float* out, cudaStream_t stream) {
+                              float scale, int mode, float* out, float* ws, long long* ws_floats,
+                              cudaStream_t stream) {
   if (B <= 0 || HW <= 0 || C <= 0 || (C % 8) || (x_Cs % 8) || (y_Cs % 8) || x_Cs < C || y_Cs < C || mode < 0 || mode > 1) {
     set_error("pair_loss_nhwc_fwd: bad arguments (B=%d HW=%lld C=%d x_Cs=%d y_Cs=%d)", B, HW, C, x_Cs, y_Cs);
     return -1;
   }
   const long long total = static_cast<long long>(B) * HW * (C / 8);
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > num_sms() * 8ll) blocks = num_sms() * 8ll;
+  const int wc = workspace_check(ws, ws_floats, blocks, "pair_loss_nhwc_fwd");
+  if (wc) return wc < 0 ? -1 : 0;
+  float* part = ws;
   pair_loss_nhwc_fwd_kernel<<<static_cast<int>(blocks), 256, 0, stream>>>(
-      static_cast<const uint16_t*>(x), x_Cs, static_cast<const uint16_t*>(y), y_Cs, w, B, HW, C / 8, scale, mode, out);
+      static_cast<const uint16_t*>(x), x_Cs, static_cast<const uint16_t*>(y), y_Cs, w, B, HW, C / 8, scale, mode, part);
   COCOS_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return ordered_sum(part, static_cast<int>(blocks), 1, out, 1, stream);  // out += the loss
 }
 
 int pair_loss_nhwc_bwd_launch(const void* x, int x_Cs, const void* y, int y_Cs, const float* w, int B, long long HW, int C,
@@ -1211,21 +1244,24 @@ int maxpool2_nhwc_bwd_launch(const void* dy, const void* x, void* dx, int B, int
   return 0;
 }
 
-int colsum_nhwc_launch(const void* x, int kind, int Cs, int C, long long rows, float* out, cudaStream_t stream) {
+int colsum_nhwc_launch(const void* x, int kind, int Cs, int C, long long rows, float* out, float* ws,
+                       long long* ws_floats, cudaStream_t stream) {
   if (C <= 0 || (C % 4) || (Cs % 4) || rows <= 0 || kind < 1 || kind > 3) {
     set_error("colsum_nhwc: bad arguments (C=%d Cs=%d rows=%lld)", C, Cs, rows);
     return -1;
   }
-  COCOS_CUDA_CHECK(cudaMemsetAsync(out, 0, sizeof(float) * C, stream));
   const int cg = (C + 127) / 128;
-  long long chunks = (4 * 148 + cg - 1) / cg;
+  long long chunks = (4ll * num_sms() + cg - 1) / cg;
   const long long max_chunks = (rows + 63) / 64;
   if (chunks > max_chunks) chunks = max_chunks;
   const int rpb = static_cast<int>((rows + chunks - 1) / chunks);
   dim3 grid(static_cast<unsigned>((rows + rpb - 1) / rpb), cg);
-  colsum_nhwc_kernel<<<grid, dim3(32, 8), 0, stream>>>(x, kind, Cs, C, rows, rpb, out);
+  const int wc = workspace_check(ws, ws_floats, static_cast<long long>(grid.x) * C, "colsum_nhwc");
+  if (wc) return wc < 0 ? -1 : 0;
+  float* part = ws;
+  colsum_nhwc_kernel<<<grid, dim3(32, 8), 0, stream>>>(x, kind, Cs, C, rows, rpb, part);
   COCOS_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return ordered_sum(part, grid.x, C, out, 0, stream);
 }
 
 int pack_w_launch(const float* w, int Cout, int Cin, int KS, void* dst, int rows, int rows_alloc, int Kc, int ngroups,

@@ -1,9 +1,9 @@
-// Plain batched tcgen05 GEMM for sm_100a:
+// Plain batched wgmma GEMM for sm_90a:
 //   C[b] (M x N fp32, row-major) = alpha * A[b] (M x K fp16) * B[b]^T (N x K fp16)  [+ C]
 // Both operands K-contiguous ("K-major"), staged by TMA into 128B-swizzled
-// shared memory; 128x128 output tile per CTA, 64-wide K chunks through a
-// multi-stage mbarrier ring; accumulator in TMEM.
-//   warp 4: TMA producer, warp 5: MMA issuer / TMEM owner, warps 0-3: epilogue.
+// shared memory; 128 x BN output tile per CTA, 64-wide K chunks through a
+// multi-stage mbarrier ring; accumulators in the registers of two warpgroups.
+//   warp 8: TMA producer, warps 0-7: wgmma (64 rows each) + epilogue.
 // Used by the correspondence backward (dQ = dS K, dK = dS^T Q) and by the
 // SAGAN-attention / 1x1-conv paths.
 #include "corr_kernels.h"
@@ -19,7 +19,7 @@ namespace {
 constexpr int BM = 128, BK = 64;
 constexpr int ATOM_BYTES = 128 * BK * 2;
 constexpr int MAX_STAGES = 6;
-constexpr int NUM_THREADS = 192;
+constexpr int NUM_THREADS = TILE_THREADS;
 
 struct GemmParams {
   int M, N, K, ldc;
@@ -33,9 +33,6 @@ struct GemmParams {
 struct GemmBars {
   uint64_t full[MAX_STAGES];
   uint64_t empty[MAX_STAGES];
-  uint64_t acc_full;
-  uint32_t tmem_base;
-  uint32_t pad;
 };
 
 template <int BN>
@@ -56,25 +53,17 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant_
   if (tid == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(smem_u32(&bars->full[i]), 1);
-      mbar_init(smem_u32(&bars->empty[i]), 1);
+      mbar_init(smem_u32(&bars->empty[i]), CONSUMER_WARPS);
     }
-    mbar_init(smem_u32(&bars->acc_full), 1);
     fence_mbar_init();
   }
-  if (warp == 4 && lane == 0) {
+  if (warp == CONSUMER_WARPS && lane == 0) {
     tma_prefetch_desc(&tm_a);
     tma_prefetch_desc(&tm_b);
   }
-  if (warp == 5) {
-    tmem_alloc(smem_u32(&bars->tmem_base), BN);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = bars->tmem_base;
 
-  if (warp == 4) {
+  if (warp == CONSUMER_WARPS) {
     if (lane == 0) {
       uint32_t st = 0, ph = 0;
       for (int kc = 0; kc < kc_count; ++kc) {
@@ -87,203 +76,56 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant_
       }
     }
     __syncwarp();
-  } else if (warp == 5) {
-    // warp-converged issue loop: every lane polls the barrier, one elected lane issues
-    const bool leader = elect_one();
-    const uint32_t idesc = make_idesc_f16(BM, BN, p.bf16 != 0);
-    uint32_t st = 0, ph = 0;
-    for (int kc = 0; kc < kc_count; ++kc) {
-      mbar_wait(smem_u32(&bars->full[st]), ph);
-      tc_fence_after();
-      if (leader) {
-        const uint32_t a_addr = smem0 + st * STAGE_BYTES;
-        const uint64_t da = make_desc_k_sw128(a_addr), db = make_desc_k_sw128(a_addr + ATOM_BYTES);
-#pragma unroll
-        for (int s4 = 0; s4 < 4; ++s4)
-          umma_f16(tmem, desc_advance_k16(da, s4), desc_advance_k16(db, s4), idesc, (kc | s4) != 0 ? 1u : 0u);
-        umma_commit(smem_u32(&bars->empty[st]));
-        if (kc == kc_count - 1) umma_commit(smem_u32(&bars->acc_full));
-      }
-      __syncwarp();
-      if (++st == STAGES) { st = 0; ph ^= 1; }
-    }
   } else {
-    const int row = m0 + tid;
-    const uint32_t lane_sel = static_cast<uint32_t>(warp * 32) << 16;
-    mbar_wait(smem_u32(&bars->acc_full), 0);
-    tc_fence_after();
-    float* crow = p.c + static_cast<size_t>(bz) * p.stride_c + static_cast<size_t>(row) * p.ldc + n0;
-    const bool vec_ok = ((p.ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.c) & 15) == 0) &&
-                        ((p.stride_c & 3) == 0);
+    float d[BN / 2];
+    const uint32_t a_off = (tid >> 7) * 64 * 128;  // this warpgroup's 64 rows of the A atom
+    consume_stages<BN>(d, kc_count, STAGES, bars->full, bars->empty, p.bf16 != 0, 0,
+                       [&](uint32_t st, int k, uint64_t& da, uint64_t& db) {
+                         const uint32_t a_addr = smem0 + st * STAGE_BYTES;
+                         da = desc_advance_k16(make_desc_k_sw128(a_addr + a_off), k);
+                         db = desc_advance_k16(make_desc_k_sw128(a_addr + ATOM_BYTES), k);
+                       });
+    const float* tile = stage_acc<BN>(d, smem_gen);
+    if (warp < 4) {
+      const int row = m0 + tid;
+      const float* arow = tile + tid * (BN + 4);
+      float* crow = p.c + static_cast<size_t>(bz) * p.stride_c + static_cast<size_t>(row) * p.ldc + n0;
+      const bool vec_ok = ((p.ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.c) & 15) == 0) &&
+                          ((p.stride_c & 3) == 0);
 #pragma unroll 1
-    for (int c = 0; c < BN / 32; ++c) {
-      uint32_t r[32];
-      tmem_ld32(tmem + lane_sel + c * 32, r);
-      tmem_wait_ld();
-      if (row < p.M) {
-        const int nbase = n0 + c * 32;
-        if (vec_ok && nbase + 32 <= p.N) {
+      for (int c = 0; c < BN / 32; ++c) {
+        uint32_t r[32];
+        acc_ld32(arow + c * 32, r);
+        if (row < p.M) {
+          const int nbase = n0 + c * 32;
+          if (vec_ok && nbase + 32 <= p.N) {
 #pragma unroll
-          for (int i = 0; i < 32; i += 4) {
-            float4 v;
-            v.x = __uint_as_float(r[i]) * p.alpha;
-            v.y = __uint_as_float(r[i + 1]) * p.alpha;
-            v.z = __uint_as_float(r[i + 2]) * p.alpha;
-            v.w = __uint_as_float(r[i + 3]) * p.alpha;
-            float4* dst = reinterpret_cast<float4*>(crow + c * 32 + i);
-            if (p.accumulate) {
-              const float4 o = *dst;
-              v.x += o.x; v.y += o.y; v.z += o.z; v.w += o.w;
+            for (int i = 0; i < 32; i += 4) {
+              float4 v;
+              v.x = __uint_as_float(r[i]) * p.alpha;
+              v.y = __uint_as_float(r[i + 1]) * p.alpha;
+              v.z = __uint_as_float(r[i + 2]) * p.alpha;
+              v.w = __uint_as_float(r[i + 3]) * p.alpha;
+              float4* dst = reinterpret_cast<float4*>(crow + c * 32 + i);
+              if (p.accumulate) {
+                const float4 o = *dst;
+                v.x += o.x; v.y += o.y; v.z += o.z; v.w += o.w;
+              }
+              *dst = v;
             }
-            *dst = v;
-          }
-        } else {
+          } else {
 #pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            if (nbase + i < p.N) {
-              float v = __uint_as_float(r[i]) * p.alpha;
-              if (p.accumulate) v += crow[c * 32 + i];
-              crow[c * 32 + i] = v;
-            }
-          }
-        }
-      }
-    }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc(tmem, BN);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// CTA-pair variant (cta_group::2): two CTAs of a cluster (same TPC) compute a 256 x 256 tile -- each holds 128 rows of
-// A and 128 rows of the B tile; one MMA instruction issued by the leader drives both SMs' tensor cores with M = 256,
-// halving the shared-memory operand traffic per SM, which is what limits the 1-CTA M = 128 instruction to ~55-75 % of
-// the tensor rate (profiles/r01_gemm_n128_vs_n256.txt).  Both CTAs run their own TMA producer and epilogue.
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NUM_THREADS, 1)
-gemm_f16_2cta_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
-                     const GemmParams p) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t smem0 = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* smem_gen = smem_raw + (smem0 - smem_u32(smem_raw));
-  constexpr int BN = 256, STAGES = 6;
-  constexpr int STAGE_BYTES = 2 * ATOM_BYTES;  // per CTA: 128 rows of A + 128 rows of B
-  GemmBars* bars = reinterpret_cast<GemmBars*>(smem_gen + STAGES * STAGE_BYTES);
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN, bz = blockIdx.z;
-  const int kc_count = (p.K + BK - 1) / BK;
-
-  if (tid == 0) {
-    for (int i = 0; i < STAGES; ++i) {
-      mbar_init(smem_u32(&bars->full[i]), 1);
-      mbar_init(smem_u32(&bars->empty[i]), 1);
-    }
-    mbar_init(smem_u32(&bars->acc_full), 1);
-    fence_mbar_init();
-  }
-  if (warp == 4 && lane == 0) {
-    tma_prefetch_desc(&tm_a);
-    tma_prefetch_desc(&tm_b);
-  }
-  cluster_sync_all();  // the peer's barriers exist before anything is signalled on them
-  if (warp == 5) {
-    tmem_alloc_2sm(smem_u32(&bars->tmem_base), BN);
-    tmem_relinquish_2sm();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = bars->tmem_base;
-
-  if (warp == 4) {
-    if (lane == 0) {
-      uint32_t st = 0, ph = 0;
-      for (int kc = 0; kc < kc_count; ++kc) {
-        mbar_wait(smem_u32(&bars->empty[st]), ph ^ 1);
-        // both halves are counted on the LEADER's barrier: it alone waits for the stage
-        const uint32_t full_leader = mapa_shared(smem_u32(&bars->full[st]), 0);
-        if (rank == 0) mbar_expect_tx(smem_u32(&bars->full[st]), 2 * STAGE_BYTES);
-        tma_load_3d_2sm(smem0 + st * STAGE_BYTES, &tm_a, full_leader, kc * BK, m0, bz);
-        tma_load_3d_2sm(smem0 + st * STAGE_BYTES + ATOM_BYTES, &tm_b, full_leader, kc * BK, n0 + rank * 128, bz);
-        if (++st == STAGES) { st = 0; ph ^= 1; }
-      }
-    }
-    __syncwarp();
-  } else if (warp == 5) {
-    if (rank == 0) {
-      const bool leader = elect_one();
-      const uint32_t idesc = make_idesc_f16(256, BN, p.bf16 != 0);
-      uint32_t st = 0, ph = 0;
-      for (int kc = 0; kc < kc_count; ++kc) {
-        mbar_wait(smem_u32(&bars->full[st]), ph);
-        tc_fence_after();
-        if (leader) {
-          const uint32_t a_addr = smem0 + st * STAGE_BYTES;
-          const uint64_t da = make_desc_k_sw128(a_addr), db = make_desc_k_sw128(a_addr + ATOM_BYTES);
-#pragma unroll
-          for (int s4 = 0; s4 < 4; ++s4)
-            umma_f16_2sm(tmem, desc_advance_k16(da, s4), desc_advance_k16(db, s4), idesc, (kc | s4) != 0 ? 1u : 0u);
-          umma_commit_2sm(smem_u32(&bars->empty[st]));
-          if (kc == kc_count - 1) umma_commit_2sm(smem_u32(&bars->acc_full));
-        }
-        __syncwarp();
-        if (++st == STAGES) { st = 0; ph ^= 1; }
-      }
-    }
-  } else {
-    const int row = m0 + tid;
-    const uint32_t lane_sel = static_cast<uint32_t>(warp * 32) << 16;
-    mbar_wait(smem_u32(&bars->acc_full), 0);
-    tc_fence_after();
-    float* crow = p.c + static_cast<size_t>(bz) * p.stride_c + static_cast<size_t>(row) * p.ldc + n0;
-    const bool vec_ok = ((p.ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.c) & 15) == 0) &&
-                        ((p.stride_c & 3) == 0);
-#pragma unroll 1
-    for (int c = 0; c < BN / 32; ++c) {
-      uint32_t r[32];
-      tmem_ld32(tmem + lane_sel + c * 32, r);
-      tmem_wait_ld();
-      if (row < p.M) {
-        const int nbase = n0 + c * 32;
-        if (vec_ok && nbase + 32 <= p.N) {
-#pragma unroll
-          for (int i = 0; i < 32; i += 4) {
-            float4 v;
-            v.x = __uint_as_float(r[i]) * p.alpha;
-            v.y = __uint_as_float(r[i + 1]) * p.alpha;
-            v.z = __uint_as_float(r[i + 2]) * p.alpha;
-            v.w = __uint_as_float(r[i + 3]) * p.alpha;
-            float4* dst = reinterpret_cast<float4*>(crow + c * 32 + i);
-            if (p.accumulate) {
-              const float4 o = *dst;
-              v.x += o.x; v.y += o.y; v.z += o.z; v.w += o.w;
-            }
-            *dst = v;
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            if (nbase + i < p.N) {
-              float v = __uint_as_float(r[i]) * p.alpha;
-              if (p.accumulate) v += crow[c * 32 + i];
-              crow[c * 32 + i] = v;
+            for (int i = 0; i < 32; ++i) {
+              if (nbase + i < p.N) {
+                float v = __uint_as_float(r[i]) * p.alpha;
+                if (p.accumulate) v += crow[c * 32 + i];
+                crow[c * 32 + i] = v;
+              }
             }
           }
         }
       }
     }
-    tc_fence_before();
-  }
-  __syncthreads();
-  cluster_sync_all();  // the peer may still be reading / the leader's MMAs may still target this CTA's TMEM
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem, BN);
   }
 }
 
@@ -309,23 +151,6 @@ int gemm_f16_launch(const void* a, const void* b, float* c, int batch, int M, in
     const char* e = getenv("COCOS_GEMM_BN");
     return (e && atoi(e) == 128) ? 128 : 256;
   }();
-  static const int two_cta = [] {
-    const char* e = getenv("COCOS_GEMM_2CTA");
-    return (e && atoi(e) == 1) ? 1 : 0;
-  }();
-  if (two_cta && N > 128 && M > 128) {
-    // CTA pairs: the B tile of 256 rows is loaded as two boxes of 128 rows, one per CTA
-    if ((rc = make_tmap_f16_3d(&tm_b, b, K, N, batch, (uint64_t)ldb * 2, sb, BK, 128, 1))) return rc;
-    GemmParams p2;
-    p2.M = M; p2.N = N; p2.K = K; p2.ldc = ldc; p2.stride_c = stride_c; p2.alpha = alpha; p2.accumulate = accumulate;
-    p2.bf16 = bf16; p2.c = c;
-    const int smem2 = 1024 + 196608 + 256;
-    const int mt = ((M + BM - 1) / BM + 1) / 2 * 2;  // an even number of M tiles: whole CTA pairs
-    COCOS_CUDA_CHECK(cudaFuncSetAttribute(gemm_f16_2cta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem2));
-    gemm_f16_2cta_kernel<<<dim3(mt, (N + 255) / 256, batch), NUM_THREADS, smem2, stream>>>(tm_a, tm_b, p2);
-    COCOS_CUDA_CHECK(cudaGetLastError());
-    return 0;
-  }
   const int BN = (bn == 256 && N > 128) ? 256 : 128;
   if ((rc = make_tmap_f16_3d(&tm_b, b, K, N, batch, (uint64_t)ldb * 2, sb, BK, BN, 1))) return rc;
   GemmParams p;

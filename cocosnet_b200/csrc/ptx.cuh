@@ -1,12 +1,14 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (alloc / mma / commit / ld / st / fences) and the shared-memory
-// matrix descriptors tcgen05.mma consumes.  No CUTLASS dependency.
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor),
+// wgmma (fence / commit / wait, accumulator staging) and the shared-memory
+// matrix descriptors wgmma consumes.  No CUTLASS dependency.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+
+#include "wgmma_ops.cuh"
 
 namespace cocos {
 
@@ -53,6 +55,13 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     }
   }
 }
+// The same bound without the report: no call inside a wgmma main loop (a call serialises the wgmma pipeline).
+__device__ __forceinline__ void mbar_wait_quiet(uint32_t bar, uint32_t parity) {
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if (++spins > COCOS_MBAR_SPIN_LIMIT) __trap();
+  }
+}
 
 // ----------------------------------------------------------------------- TMA
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
@@ -74,180 +83,116 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* m, 
       "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
-// generic-proxy smem writes -> visible to the async proxy (tcgen05.mma / TMA)
+// generic-proxy smem writes -> visible to the async proxy (wgmma / TMA)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
-// ------------------------------------------------------------------- tcgen05
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols)
-               : "memory");
+// -------------------------------------------------------------------- wgmma
+// Warpgroup MMA (sm_90a): D (registers, fp32) (+)= A * B over a 64-row slab per warpgroup; see wgmma_ops.cuh.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T ; kind::f16 (fp16/bf16 in, fp32 accumulate)
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]^T : A operand read from tensor memory (lane = row, each 32-bit column holds two
-// consecutive-K 16-bit elements)
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier once every tcgen05 op issued so far by this thread
-// has completed (implies tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 bit, 32 consecutive columns: thread t of the warp gets lane
-// (warp%4)*32+t, registers r[0..31] = columns col..col+31.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-      "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-      "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-      "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-      "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
+// keep the compiler from moving accumulator reads / writes across an in-flight wgmma
+template <int R>
+__device__ __forceinline__ void reg_fence(float* d) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ------------------------------------------------------------ CTA pairs (cta_group::2)
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
+// named barrier over `n` threads (id 0 is __syncthreads)
+__device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+
+// Accumulator fragment of m64nN (thread t of the warpgroup: rows 16*(t/32) + (t%32)/4 and +8, column pairs
+// 8j + 2*(t%4)) -> row-major fp32 tile rows [row0, row0 + 64), pitch `ld` floats (even).
+template <int N>
+__device__ __forceinline__ void acc_to_smem(const float* d, float* tile, int ld, int row0) {
+  const int t = threadIdx.x & 127;
+  const int r = row0 + 16 * (t >> 5) + ((t & 31) >> 2), c = 2 * (t & 3);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    *reinterpret_cast<float2*>(tile + r * ld + 8 * j + c) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(tile + (r + 8) * ld + 8 * j + c) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
 }
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of the same shared-memory variable in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t local_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(rank));
-  return r;
-}
-// remote arrive on an mbarrier of another CTA of the cluster (address from mapa_shared)
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA load of a CTA pair: the data lands in THIS CTA's shared memory, the bytes are signalled on `bar`, a
-// shared::cluster address that may belong to the peer (the leader CTA waits once for both halves of an operand)
-__device__ __forceinline__ void tma_load_3d_2sm(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1,
-                                                int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes "
-      "[%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A * B^T with M = 256 over the CTA pair (each CTA holds 128 rows of A and N/2 rows of B at
-// the same shared-memory offsets); issued by the leader CTA only
-__device__ __forceinline__ void umma_f16_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on the mbarrier at this shared-memory offset in BOTH CTAs once the tcgen05 ops issued so far completed
-__device__ __forceinline__ void umma_commit_2sm(uint32_t bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-      "h"(static_cast<uint16_t>(3))
-      : "memory");
+// 32 consecutive fp32 of a staged accumulator row (16-byte aligned) as raw bits
+__device__ __forceinline__ void acc_ld32(const float* src, uint32_t* r) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const float4 v = reinterpret_cast<const float4*>(src)[i];
+    r[4 * i] = __float_as_uint(v.x); r[4 * i + 1] = __float_as_uint(v.y);
+    r[4 * i + 2] = __float_as_uint(v.z); r[4 * i + 3] = __float_as_uint(v.w);
+  }
 }
 
 // --------------------------------------------------------------- descriptors
-// K-major operand tile staged by TMA with SWIZZLE_128B: rows of 64 fp16
-// (128 B), 8-row groups 1024 B apart.  (cute/arch/mma_sm100_desc.hpp:
-// start[0,14) lbo[16,30) sbo[32,46) version[46,48)=1 layout[61,64)=2.)
+// K-major operand tile staged by TMA with SWIZZLE_128B: rows of 64 16-bit elements (128 B), 8-row groups 1024 B apart.
+// wgmma matrix descriptor: start[0,14) lbo[16,30) sbo[32,46) layout[62,64)=1 (128B swizzle), addresses in 16 B units.
 __device__ __forceinline__ uint64_t make_desc_k_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(1) << 16;            // leading byte offset (unused for swizzled K-major)
   d |= static_cast<uint64_t>(1024 >> 4) << 32;    // stride byte offset: 8 rows * 128 B
-  d |= static_cast<uint64_t>(1) << 46;            // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;            // SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;            // SWIZZLE_128B
   return d;
 }
-// instruction descriptor, kind::f16: A,B fp16 (format 0) K-major, D fp32.
-__host__ __device__ constexpr uint32_t make_idesc_f16(int m, int n, bool bf16 = false) {
-  return (1u << 4) | ((bf16 ? 1u : 0u) << 7) | ((bf16 ? 1u : 0u) << 10) | (static_cast<uint32_t>(n >> 3) << 17) |
-         (static_cast<uint32_t>(m >> 4) << 24);
+// MN-major operand, SWIZZLE_128B: 64-element (128 B) rows along MN, 8 K-rows 1024 B apart (SBO), the next 64-element
+// block along MN `lbo_bytes` further.
+__device__ __forceinline__ uint64_t make_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
+  d |= static_cast<uint64_t>(lbo_bytes >> 4) << 16;
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;
+  d |= static_cast<uint64_t>(1) << 62;
+  return d;
 }
 
 // descriptor for the next 16-element K step inside a 128B swizzle atom (+32 bytes)
 __device__ __forceinline__ uint64_t desc_advance_k16(uint64_t d, int steps) { return d + static_cast<uint64_t>(2 * steps); }
+
+// ------------------------------------------------------- 128-row tile main loop
+// The GEMM-like kernels run two consumer warpgroups (warps 0-7; warpgroup g owns accumulator rows [64g, 64g + 64))
+// and one TMA producer warp (warp 8).  Stage `st` of the ring is released with one arrive per consumer warp, so the
+// `empty` barriers are initialised with CONSUMER_WARPS.
+constexpr int CONSUMER_WARPS = 8;
+constexpr int TILE_THREADS = 32 * CONSUMER_WARPS + 32;
+
+// d (+)= sum over `iters` stages of 4 K16 steps; desc(st, k, da, db) gives this warpgroup's descriptors.
+template <int BN, typename Desc>
+__device__ __forceinline__ void consume_stages(float* d, int iters, int stages, uint64_t* full, uint64_t* empty,
+                                               bool bf16, int tnsp, Desc desc) {
+  uint32_t st = 0, ph = 0;
+  for (int it = 0; it < iters; ++it) {
+    mbar_wait_quiet(smem_u32(&full[st]), ph);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      uint64_t da, db;
+      desc(st, k, da, db);
+      if (bf16) wgmma_ss<BN, true>(d, da, db, (it | k) != 0 ? 1 : 0, tnsp);
+      else wgmma_ss<BN, false>(d, da, db, (it | k) != 0 ? 1 : 0, tnsp);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(smem_u32(&empty[st]));
+    if (++st == static_cast<uint32_t>(stages)) { st = 0; ph ^= 1; }
+  }
+}
+
+// After the main loop: both warpgroups write their accumulators into the (drained) operand ring as a row-major fp32
+// tile of 128 rows, pitch BN + 4, for an epilogue that reads one row per thread.
+template <int BN>
+__device__ __forceinline__ float* stage_acc(const float* d, uint8_t* ring) {
+  float* tile = reinterpret_cast<float*>(ring);
+  bar_sync(1, 32 * CONSUMER_WARPS);  // every consumer warp is past its last wgmma on the ring
+  acc_to_smem<BN>(d, tile, BN + 4, 64 * (threadIdx.x >> 7));
+  bar_sync(1, 32 * CONSUMER_WARPS);
+  return tile;
+}
 
 // one lane of a converged warp
 __device__ __forceinline__ bool elect_one() {

@@ -6,12 +6,13 @@
 //     v <- normalize(W^T u),  u <- normalize(W v),  sigma = u^T W v,  weight = weight_orig / sigma
 // -- about ten small launches per layer, ~100 layer invocations per training iteration.  Here a device-resident table
 // lists the layers of one network forward and each phase is ONE launch over all of them:
-//   phase A: t = W^T u (column sums, coalesced), |t|^2 accumulated per layer       -> v holds t
-//   phase B: s = W t / max(|t|, eps) (one warp per row), |s|^2 accumulated         -> u holds s
+//   phase A: t = W^T u (column sums, coalesced), |t|^2 partial per block            -> v holds t
+//   phase B: s = W t / max(|t|, eps) (one warp per row), |s|^2 partial per block    -> u holds s
 //   phase C: v = t / max(|t|, eps), u = s / max(|s|, eps), inv_sigma = 1 / (u^T W v) = max(|s|, eps) / |s|^2
 // (u^T W v = u^T s = |s|^2 / max(|s|, eps)).  The division weight_orig / sigma never happens: the convolution kernels
 // take inv_sigma as an epilogue scale.  Evaluation mode (no power iteration): phase B' computes W v with the stored v
-// and phase C' only the dot product with the stored u.
+// and phase C' only the dot product with the stored u.  The per-block partials go to a workspace and are added per layer
+// in block order (no floating-point atomics): the same weights give the same sigma on every call.
 #include "corr_kernels.h"
 #include "tmap.h"
 
@@ -38,7 +39,7 @@ __device__ __forceinline__ int find_entry(const SnEntry* __restrict__ tab, int n
 
 // phase A: block = 128 columns (32 threads x 4) x 8 row lanes
 __global__ void __launch_bounds__(256)
-sn_cols_kernel(const SnEntry* __restrict__ tab, int n, float* __restrict__ scratch) {
+sn_cols_kernel(const SnEntry* __restrict__ tab, int n, float* __restrict__ part_a) {
   __shared__ float red[8][32][4];
   const int e = find_entry(tab, n, blockIdx.x, false);
   const SnEntry L = tab[e];
@@ -76,14 +77,22 @@ sn_cols_kernel(const SnEntry* __restrict__ tab, int n, float* __restrict__ scrat
       }
     }
     sq = warp_sum_sn(sq);
-    if (tx == 0) atomicAdd(scratch + 2 * e, sq);
+    if (tx == 0) part_a[blockIdx.x] = sq;
   }
+}
+
+// |t|^2 of layer L: its phase-A partials in block order
+__device__ __forceinline__ float sum_t2(const SnEntry& L, const float* __restrict__ part_a) {
+  float t2 = 0.f;
+  for (long long k = 0; k < (L.cols + 127) / 128; ++k) t2 += part_a[L.block_a + k];
+  return t2;
 }
 
 // phase B: one warp per row; scale_v: multiply v by 1 / max(|t|, eps) on the fly (training) or use it as stored
 __global__ void __launch_bounds__(256)
-sn_rows_kernel(const SnEntry* __restrict__ tab, int n, float* __restrict__ scratch, float eps, int scale_v,
-               float* __restrict__ rows_out_eval) {
+sn_rows_kernel(const SnEntry* __restrict__ tab, int n, const float* __restrict__ part_a, float* __restrict__ part_b,
+               float eps, int scale_v) {
+  __shared__ float red[8];
   const int e = find_entry(tab, n, blockIdx.x, true);
   const SnEntry L = tab[e];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -102,34 +111,50 @@ sn_rows_kernel(const SnEntry* __restrict__ tab, int n, float* __restrict__ scrat
     }
   }
   acc = warp_sum_sn(acc);
+  float contrib = 0.f;
   if (r < L.rows && lane == 0) {
     if (scale_v) {
-      const float s = acc / fmaxf(sqrtf(scratch[2 * e]), eps);
+      const float s = acc / fmaxf(sqrtf(sum_t2(L, part_a)), eps);
       L.u[r] = s;  // unnormalised W v
-      atomicAdd(scratch + 2 * e + 1, s * s);
+      contrib = s * s;
     } else {
-      atomicAdd(scratch + 2 * e + 1, acc * L.u[r]);  // u^T (W v) with the stored u, v
+      contrib = acc * L.u[r];  // u^T (W v) with the stored u, v
     }
   }
-  (void)rows_out_eval;
+  if (lane == 0) red[warp] = contrib;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float t = 0.f;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) t += red[k];
+    part_b[blockIdx.x] = t;
+  }
 }
 
 // phase C: normalise u, v in place and emit 1 / sigma; one block per layer
 // `snapshot` (may be NULL) receives a copy [u | v] of the vectors sigma was computed with: the backward of THIS forward
 // needs them (d sigma / dW = u v^T) after later forwards of the same layer have advanced the persistent ones.
 __global__ void __launch_bounds__(256)
-sn_finish_kernel(const SnEntry* __restrict__ tab, const float* __restrict__ scratch, float eps, int training,
-                 float* __restrict__ inv_sigma, float* __restrict__ snapshot) {
+sn_finish_kernel(const SnEntry* __restrict__ tab, const float* __restrict__ part_a, const float* __restrict__ part_b,
+                 float* __restrict__ scratch, float eps, int training, float* __restrict__ inv_sigma,
+                 float* __restrict__ snapshot) {
   const int e = blockIdx.x;
   const SnEntry L = tab[e];
+  float sb = 0.f;  // |s|^2 (training) or u^T W v (evaluation): the layer's phase-B partials in block order
+  for (long long k = 0; k < (L.rows + 7) / 8; ++k) sb += part_b[L.block_b + k];
+  const float t2 = training ? sum_t2(L, part_a) : 0.f;
+  if (threadIdx.x == 0) {
+    scratch[2 * e] = t2;
+    scratch[2 * e + 1] = sb;
+  }
   float tn = 1.f, sn = 1.f;
   if (training) {
-    tn = fmaxf(sqrtf(scratch[2 * e]), eps);
-    const float sn2 = scratch[2 * e + 1];
+    tn = fmaxf(sqrtf(t2), eps);
+    const float sn2 = sb;
     sn = fmaxf(sqrtf(sn2), eps);
     if (threadIdx.x == 0) inv_sigma[e] = sn / sn2;
   } else if (threadIdx.x == 0) {
-    inv_sigma[e] = 1.0f / scratch[2 * e + 1];
+    inv_sigma[e] = 1.0f / sb;
   }
   float* su = snapshot ? snapshot + L.snap : nullptr;
   for (long long r = threadIdx.x; r < L.rows; r += 256) {
@@ -153,10 +178,11 @@ int sn_power_iter_launch(const void* table, int n, int blocks_a, int blocks_b, f
     return -1;
   }
   const SnEntry* tab = static_cast<const SnEntry*>(table);
-  COCOS_CUDA_CHECK(cudaMemsetAsync(scratch, 0, sizeof(float) * 2 * n, stream));
-  if (training) sn_cols_kernel<<<blocks_a, 256, 0, stream>>>(tab, n, scratch);
-  sn_rows_kernel<<<blocks_b, 256, 0, stream>>>(tab, n, scratch, eps, training, nullptr);
-  sn_finish_kernel<<<n, 256, 0, stream>>>(tab, scratch, eps, training, inv_sigma, snapshot);
+  float* part_a = scratch + 2 * n;  // per-block partials of phase A, then of phase B
+  float* part_b = part_a + blocks_a;
+  if (training) sn_cols_kernel<<<blocks_a, 256, 0, stream>>>(tab, n, part_a);
+  sn_rows_kernel<<<blocks_b, 256, 0, stream>>>(tab, n, part_a, part_b, eps, training);
+  sn_finish_kernel<<<n, 256, 0, stream>>>(tab, part_a, part_b, scratch, eps, training, inv_sigma, snapshot);
   COCOS_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

@@ -1,4 +1,4 @@
-// K2n: persistent TMA-fed tcgen05 implicit-GEMM "tap convolution" over 16-bit NHWC activations, sm_100a.
+// K2n: TMA-fed wgmma implicit-GEMM "tap convolution" over 16-bit NHWC activations, sm_90a.
 //
 //   Y[b, h, w, n] = epilogue( sum_{g < ngroups} sum_{c < 64*kchunks}
 //                             X[b, s*h + dh[g], s*w + dw[g], coff[g] + c] * Wt[n, (g*kchunks)*64 + c] )
@@ -15,14 +15,14 @@
 // Operands:
 //   * A tile = ONE 5-D TMA box {64 ch, TW, 1, TH, TB} of the activation tensor seen as
 //     [B, Hin/s, s (row parity), Win/s, s (col parity) * Ca]: its TB*TH*TW rows of 128 B land pixel after pixel with
-//     the 128B swizzle, i.e. directly in the K-major operand layout of tcgen05.mma (no im2col, no strided gather:
+//     the 128B swizzle, i.e. directly in the K-major operand layout of wgmma (no im2col, no strided gather:
 //     a stride-2 tap is a plain tile of the parity-split view).  Out-of-image taps and channels >= Ca are TMA
 //     zero fill (zero padding for free; reflection halos are materialised by the producing epilogue).
 //   * B tile = weights [Cout, ngroups*kchunks*64] K-major, box {64, BN}.
-//   * accumulators: TWO TMEM buffers of BN fp32 columns; the epilogue of tile i overlaps the main loop of tile i+1.
+//   * accumulators: registers of two warpgroups (64 rows x BN fp32 each), staged through shared memory for the epilogue.
 // Epilogue (4 warps, one thread per output pixel): + bias, + residual, activation, then store as fp16 / bf16 / fp32
 // NHWC (optionally with a 1-pixel halo filled by reflection, optionally as a 2-term [hi | lo] split) or fp32 NCHW.
-// warp 4: TMA producer, warp 5: MMA issuer (UMMA M=128, N=BN), warps 0-3: epilogue.  Grid = min(#tiles, #SMs).
+// warp 8: TMA producer, warps 0-7: wgmma (M=64 each, N=BN), warps 0-3: epilogue.  One CTA per output tile.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -37,7 +37,7 @@ namespace {
 
 constexpr int BM = 128, BK = 64;
 constexpr int ATOM_BYTES = 128 * BK * 2;
-constexpr int NUM_THREADS = 192;
+constexpr int NUM_THREADS = TILE_THREADS;
 constexpr int MAXG = COCOS_TAPCONV_MAX_GROUPS;
 
 struct TapParams {
@@ -67,10 +67,6 @@ struct TapParams {
 struct TapBars {
   uint64_t full[6];
   uint64_t empty[6];
-  uint64_t acc_full[2];
-  uint64_t acc_empty[2];
-  uint32_t tmem_base;
-  uint32_t pad;
 };
 
 __device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2,
@@ -148,97 +144,67 @@ tapconv_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
   if (tid == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(smem_u32(&bars->full[i]), 1);
-      mbar_init(smem_u32(&bars->empty[i]), 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(smem_u32(&bars->acc_full[i]), 1);
-      mbar_init(smem_u32(&bars->acc_empty[i]), 4);  // one arrive per epilogue warp
+      mbar_init(smem_u32(&bars->empty[i]), CONSUMER_WARPS);
     }
     fence_mbar_init();
   }
-  if (warp == 4 && lane == 0) {
+  if (warp == CONSUMER_WARPS && lane == 0) {
     tma_prefetch_desc(&tm_x);
     tma_prefetch_desc(&tm_w);
   }
-  if (warp == 5) {
-    tmem_alloc(smem_u32(&bars->tmem_base), 2 * BN);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = bars->tmem_base;
 
-  if (warp == 4) {
+  const int tile = blockIdx.x;
+  if (warp == CONSUMER_WARPS) {
     // ------------------------------------------------------------------ TMA producer
     if (elect_one()) {
       uint32_t st = 0, ph = 0;
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-        int t = tile;
-        const int n_i = t % p.tiles_n; t /= p.tiles_n;
-        const int tw_i = t % p.tiles_w; t /= p.tiles_w;
-        const int th_i = t % p.tiles_h;
-        const int tb_i = t / p.tiles_h;
-        const int h0 = th_i * p.TH, w0 = tw_i * p.TW, b0 = tb_i * p.TB, n0 = n_i * BN;
-        for (int g = 0; g < p.ngroups; ++g) {
-          int dh = p.dh[g], dw = p.dw[g], hpar = 0, cbase = p.coff[g];
-          if (p.a_stride == 2) {
-            hpar = dh & 1;
-            dh = floordiv2(dh);
-            cbase += (dw & 1) * p.Ca;
-            dw = floordiv2(dw);
-          }
-          for (int kc = 0; kc < p.kchunks; ++kc) {
-            mbar_wait(smem_u32(&bars->empty[st]), ph ^ 1);
-            const uint32_t full = smem_u32(&bars->full[st]);
-            mbar_expect_tx(full, a_bytes + (BN / 128) * ATOM_BYTES);
-            tma_load_5d(smem0 + st * STAGE_BYTES, &tm_x, full, cbase + kc * BK, w0 + dw, hpar, h0 + dh, b0);
-            tma_load_3d(smem0 + st * STAGE_BYTES + ATOM_BYTES, &tm_w, full, (g * p.kchunks + kc) * BK, n0, 0);
-            if (++st == STAGES) { st = 0; ph ^= 1; }
-          }
+      int t = tile;
+      const int n_i = t % p.tiles_n; t /= p.tiles_n;
+      const int tw_i = t % p.tiles_w; t /= p.tiles_w;
+      const int th_i = t % p.tiles_h;
+      const int tb_i = t / p.tiles_h;
+      const int h0 = th_i * p.TH, w0 = tw_i * p.TW, b0 = tb_i * p.TB, n0 = n_i * BN;
+      for (int g = 0; g < p.ngroups; ++g) {
+        int dh = p.dh[g], dw = p.dw[g], hpar = 0, cbase = p.coff[g];
+        if (p.a_stride == 2) {
+          hpar = dh & 1;
+          dh = floordiv2(dh);
+          cbase += (dw & 1) * p.Ca;
+          dw = floordiv2(dw);
         }
-      }
-    }
-  } else if (warp == 5) {
-    // ------------------------------------------------------------------ MMA issuer
-    const bool leader = elect_one();
-    const uint32_t idesc = make_idesc_f16(BM, BN, p.bf16 != 0);
-    uint32_t st = 0, ph = 0;
-    int local = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++local) {
-      const int buf = local & 1;
-      mbar_wait(smem_u32(&bars->acc_empty[buf]), ((local >> 1) & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t acc = tmem + buf * BN;
-      for (int it = 0; it < iters; ++it) {
-        mbar_wait(smem_u32(&bars->full[st]), ph);
-        tc_fence_after();
-        if (leader) {
-          const uint32_t a_addr = smem0 + st * STAGE_BYTES;
-          const uint64_t da = make_desc_k_sw128(a_addr), db = make_desc_k_sw128(a_addr + ATOM_BYTES);
-#pragma unroll
-          for (int s4 = 0; s4 < 4; ++s4)
-            umma_f16(acc, desc_advance_k16(da, s4), desc_advance_k16(db, s4), idesc, (it | s4) != 0 ? 1u : 0u);
-          umma_commit(smem_u32(&bars->empty[st]));
-          if (it == iters - 1) umma_commit(smem_u32(&bars->acc_full[buf]));
+        for (int kc = 0; kc < p.kchunks; ++kc) {
+          mbar_wait(smem_u32(&bars->empty[st]), ph ^ 1);
+          const uint32_t full = smem_u32(&bars->full[st]);
+          mbar_expect_tx(full, a_bytes + (BN / 128) * ATOM_BYTES);
+          tma_load_5d(smem0 + st * STAGE_BYTES, &tm_x, full, cbase + kc * BK, w0 + dw, hpar, h0 + dh, b0);
+          tma_load_3d(smem0 + st * STAGE_BYTES + ATOM_BYTES, &tm_w, full, (g * p.kchunks + kc) * BK, n0, 0);
+          if (++st == STAGES) { st = 0; ph ^= 1; }
         }
-        __syncwarp();
-        if (++st == STAGES) { st = 0; ph ^= 1; }
       }
     }
   } else {
+    // ------------------------------------------------------------------ wgmma main loop
+    float d[BN / 2];
+    const uint32_t a_off = (tid >> 7) * 64 * 128;
+    consume_stages<BN>(d, iters, STAGES, bars->full, bars->empty, p.bf16 != 0, 0,
+                       [&](uint32_t st, int k, uint64_t& da, uint64_t& db) {
+                         const uint32_t a_addr = smem0 + st * STAGE_BYTES;
+                         da = desc_advance_k16(make_desc_k_sw128(a_addr + a_off), k);
+                         db = desc_advance_k16(make_desc_k_sw128(a_addr + ATOM_BYTES), k);
+                       });
+    const float* acc_tile = stage_acc<BN>(d, smem_gen);
+    if (warp >= 4) return;
     // ------------------------------------------------------------------ epilogue (one thread per output pixel)
     const int m = tid;
     const int rows_per_img = p.TH * p.TW;
     const int tb = m / rows_per_img, rem = m - tb * rows_per_img;
     const int th = rem / p.TW, tw = rem - th * p.TW;
-    const uint32_t lane_sel = static_cast<uint32_t>(warp * 32) << 16;
     const int yHp = p.y_H + 2 * p.y_pad, yWp = p.y_W + 2 * p.y_pad;
     const bool out16 = p.y_kind == 1 || p.y_kind == 2;
     const bool obf = p.y_kind == 2;
     const float scale = p.scale ? __ldg(p.scale) : 1.0f;
-    int local = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++local) {
+    {
       int t = tile;
       const int n_i = t % p.tiles_n; t /= p.tiles_n;
       const int tw_i = t % p.tiles_w; t /= p.tiles_w;
@@ -258,10 +224,7 @@ tapconv_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
         if (yw == 1) ct[nc++] = 0;
         if (yw == p.y_W - 2) ct[nc++] = p.y_W + 1;
       }
-      const int buf = local & 1;
-      mbar_wait(smem_u32(&bars->acc_full[buf]), (local >> 1) & 1);
-      tc_fence_after();
-      const uint32_t acc = tmem + buf * BN + lane_sel;
+      const float* acc = acc_tile + m * (BN + 4);
       if (p.mod_W) {
         // ---- SPADE: y = reflect_pad(lrelu(PONO(x) * (1 + gamma) + beta)) straight from the gamma / beta accumulators
         // (normalization.py:132-149 + architecture.py:73-74); the raw [gamma | beta] pair is stored too when the
@@ -272,9 +235,8 @@ tapconv_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
 #pragma unroll 1
         for (int c = 0; c < p.mod_W / 32; ++c) {
           uint32_t rg[32], rb[32];
-          tmem_ld32(acc + c * 32, rg);
-          tmem_ld32(acc + p.mod_W + c * 32, rb);
-          tmem_wait_ld();
+          acc_ld32(acc + c * 32, rg);
+          acc_ld32(acc + p.mod_W + c * 32, rb);
           if (!ok) continue;
           const int ch = n_i * p.mod_W + c * 32;        // channel of x / y
           const int ng = n0 + c * 32, nbt = ng + p.mod_W;  // columns (= rows of the interleaved weight / bias)
@@ -338,18 +300,14 @@ tapconv_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
               if (p.y_lo_off) store16(static_cast<uint16_t*>(p.y) + po + p.y_lo_off, lo, 32, true, false);
             }
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&bars->acc_empty[buf]));
-        continue;
+        return;
       }
 #pragma unroll 1
       for (int c = 0; c < BN / 32; ++c) {
         const int nb = n0 + c * 32;
         if (nb >= p.Cout) break;  // uniform
         uint32_t r[32];
-        tmem_ld32(acc + c * 32, r);
-        tmem_wait_ld();
+        acc_ld32(acc + c * 32, r);
         if (!ok) continue;
         const int n_ok = min(32, p.Cout - nb);
         float v[32];
@@ -405,27 +363,8 @@ tapconv_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
             }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&bars->acc_empty[buf]));
     }
   }
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 2 * BN);
-  }
-}
-
-int num_sms() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
-        n <= 0)
-      n = 148;
-  }
-  return n;
 }
 
 }  // namespace
@@ -521,7 +460,7 @@ int tapconv_launch(const cocos_tapconv_desc* d, cudaStream_t stream) {
   const uint64_t wrows = (uint64_t)(d->w_rows >= d->Cout ? d->w_rows : d->Cout);
   if ((rc = make_tmap_f16_3d(&tm_w, d->w, Kt, wrows, 1, Kt * 2, wrows * Kt * 2, BK, BN, 1))) return rc;
   const int smem_bytes = 1024 + 196608 + 256;
-  int grid = p.num_tiles < num_sms() ? p.num_tiles : num_sms();
+  const int grid = p.num_tiles;
   if (BN == 256) {
     COCOS_CUDA_CHECK(cudaFuncSetAttribute(tapconv_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
     tapconv_kernel<256><<<grid, NUM_THREADS, smem_bytes, stream>>>(tm_x, tm_w, p);

@@ -1,22 +1,23 @@
-// K2w-n: backward-weights of the tap convolution (tapconv.cu) over 16-bit NHWC tensors, sm_100a.
+// K2w-n: backward-weights of the tap convolution (tapconv.cu) over 16-bit NHWC tensors, sm_90a.
 //
 //   dW[g, n, c] = sum_{b,h,w} dY[b, h, w, n] * X[b, s*h + dh[g], s*w + dw[g], coff + c]
 //
 // (the wgrad half of autograd's convolution_backward for every nn.Conv2d the tap convolution serves; same reference
 // call sites).  One GEMM per tap group g: M = 128 output channels n, N = 128/256 input channels c, K = pixels.
 // With NHWC activations the channels are the contiguous dimension of BOTH operands, i.e. both are "MN-major" for
-// tcgen05.mma: a K step is a run of pixels, each pixel a 128-byte row of 64 channels - exactly what the same 5-D TMA
+// wgmma: a K step is a run of pixels, each pixel a 128-byte row of 64 channels - exactly what the same 5-D TMA
 // boxes the forward kernel uses deliver ({64 ch, TW, 1, TH, 1} with TW*TH = 64 pixels, 128B swizzle), so there are no
 // transposed / shifted operand copies at all (the NCHW version needed KS shifted 16-bit copies of X per layer).
 //   * A = dY (bf16), 2 atoms of 64 channels; B = X, BN/64 atoms, the tap's offset / stride-2 parity in the coordinates;
 //     smem descriptors: MN-major, SWIZZLE_128B, LBO = bytes between 64-channel atoms (64 pixels * 128 B),
 //     SBO = 1024 B between 8-pixel groups; a K=16 step advances the start address by 16 pixels = 2048 B.
-//   * X is what the forward saved: fp16.  tcgen05 cannot mix fp16 x bf16 operands and gradients need the bf16 range,
-//     so the four otherwise idle epilogue warps convert the landed X atoms fp16 -> bf16 IN PLACE in shared memory
-//     (elementwise, so the swizzle does not matter), fence to the async proxy and hand the stage to the MMA warp.
-//   * the pixel range is split over the grid (split-K) and partial tiles are reduced with red.global.add.f32 into
-//     ws[g][n][c] (a thread owns 32 consecutive c of one n: 128-byte runs).
-// warp 4: TMA producer, warp 5: MMA issuer, warps 0-3: converter + epilogue.
+//   * X is what the forward saved: fp16.  wgmma cannot mix fp16 x bf16 operands and gradients need the bf16 range,
+//     so the consumer warps convert the landed X atoms fp16 -> bf16 IN PLACE in shared memory (elementwise, so the
+//     swizzle does not matter) and fence to the async proxy before their wgmma reads the stage.
+//   * the pixel range is split over the grid (split-K): split k stores its partial tile into slice k of a workspace
+//     and ordered_sum() adds the slices in split order into ws[g][n][c] (same bits on every run; a thread owns 32
+//     consecutive c of one n: 128-byte runs).
+// warp 8: TMA producer, warps 0-7: converter + wgmma (64 output channels each), warps 0-3: epilogue.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -32,7 +33,7 @@ namespace {
 constexpr int BM = 128;
 constexpr int KP = 64;                    // pixels per pipeline stage
 constexpr int ATOM = KP * 128;            // one 64-channel atom: 64 pixel rows of 128 B
-constexpr int NUM_THREADS = 192;
+constexpr int NUM_THREADS = TILE_THREADS;
 constexpr int MAXG = COCOS_TAPCONV_MAX_GROUPS;
 
 struct WgParams {
@@ -42,16 +43,13 @@ struct WgParams {
   int ngroups;
   int8_t dh[MAXG], dw[MAXG];
   int16_t coff[MAXG];
-  float* ws;  // [ngroups, Cout, Cin_s]
+  float* ws;  // [ngroups, Cout, Cin_s], or with splits > 1 the workspace [splits][ngroups, Cout, Cin_s]
+  long long ws_size;
 };
 
 struct WgBars {
   uint64_t full[4];
-  uint64_t conv[4];
   uint64_t empty[4];
-  uint64_t acc_full;
-  uint32_t tmem_base;
-  uint32_t pad;
 };
 
 __device__ __forceinline__ void tma_load_5d_w(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2,
@@ -63,31 +61,10 @@ __device__ __forceinline__ void tma_load_5d_w(uint32_t dst, const CUtensorMap* m
       : "memory");
 }
 
-// MN-major operand, SWIZZLE_128B: 64-element (128 B) rows, 8-row groups 1024 B apart (SBO), next 64-element atom
-// `lbo_bytes` further (cute/arch/mma_sm100_desc.hpp, make_umma_desc<Major::MN>).
-__device__ __forceinline__ uint64_t make_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(lbo_bytes >> 4) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-// kind::f16, bf16 x bf16 -> fp32, A and B MN-major (bits 15 / 16)
-__host__ __device__ constexpr uint32_t make_idesc_bf16_mn(int m, int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | (static_cast<uint32_t>(n >> 3) << 17) |
-         (static_cast<uint32_t>(m >> 4) << 24);
-}
-
 __device__ __forceinline__ uint32_t h2_to_bf2(uint32_t h) {
   const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&h));
   const __nv_bfloat162 b = __floats2bfloat162_rn(f.x, f.y);
   return *reinterpret_cast<const uint32_t*>(&b);
-}
-
-__device__ __forceinline__ void red_add_v4(float* dst, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
 
 template <int BN>
@@ -114,26 +91,17 @@ tapwgrad_kernel(const __grid_constant__ CUtensorMap tm_dy, const __grid_constant
   if (tid == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(smem_u32(&bars->full[i]), 1);
-      mbar_init(smem_u32(&bars->conv[i]), 4);
-      mbar_init(smem_u32(&bars->empty[i]), 1);
+      mbar_init(smem_u32(&bars->empty[i]), CONSUMER_WARPS);
     }
-    mbar_init(smem_u32(&bars->acc_full), 1);
     fence_mbar_init();
   }
-  if (warp == 4 && lane == 0) {
+  if (warp == CONSUMER_WARPS && lane == 0) {
     tma_prefetch_desc(&tm_dy);
     tma_prefetch_desc(&tm_x);
   }
-  if (warp == 5) {
-    tmem_alloc(smem_u32(&bars->tmem_base), BN);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = bars->tmem_base;
 
-  if (warp == 4) {
+  if (warp == CONSUMER_WARPS) {
     if (elect_one()) {
       int dh = p.dh[g], dw = p.dw[g], hpar = 0, cbase = p.coff[g] + c0;
       if (p.a_stride == 2) {
@@ -166,91 +134,72 @@ tapwgrad_kernel(const __grid_constant__ CUtensorMap tm_dy, const __grid_constant
         }
       }
     }
-  } else if (warp == 5) {
-    const bool leader = elect_one();
-    const uint32_t idesc = make_idesc_bf16_mn(BM, BN);
+  } else {
+    constexpr int CT = 32 * CONSUMER_WARPS;
+    const int wg = tid >> 7;  // output channels [n0 + 64 wg, n0 + 64 wg + 64) = dY atom wg
+    float d[BN / 2];
     uint32_t st = 0, ph = 0;
     for (int it = 0; it < iters; ++it) {
-      mbar_wait(smem_u32(p.x_f16 ? &bars->conv[st] : &bars->full[st]), ph);
-      tc_fence_after();
-      if (leader) {
-        const uint32_t a_addr = smem0 + st * STAGE_BYTES;
-        const uint64_t da = make_desc_mn_sw128(a_addr, ATOM), db = make_desc_mn_sw128(a_addr + 2 * ATOM, ATOM);
-#pragma unroll
-        for (int k = 0; k < KP / 16; ++k)  // 16 pixels = 2048 B further along K
-          umma_f16(tmem, da + static_cast<uint64_t>(k * 128), db + static_cast<uint64_t>(k * 128), idesc,
-                   (it | k) != 0 ? 1u : 0u);
-        umma_commit(smem_u32(&bars->empty[st]));
-        if (it == iters - 1) umma_commit(smem_u32(&bars->acc_full));
-      }
-      __syncwarp();
-      if (++st == STAGES) { st = 0; ph ^= 1; }
-    }
-  } else {
-    if (p.x_f16) {
-      // ---------------------------------------------------------------- converter: X atoms fp16 -> bf16 in place
-      uint32_t st = 0, ph = 0;
-      for (int it = 0; it < iters; ++it) {
-        mbar_wait(smem_u32(&bars->full[st]), ph);
+      mbar_wait_quiet(smem_u32(&bars->full[st]), ph);
+      if (p.x_f16) {
+        // ------------------------------------------------------------ converter: X atoms fp16 -> bf16 in place
         uint4* xb = reinterpret_cast<uint4*>(smem_gen + st * STAGE_BYTES + 2 * ATOM);
 #pragma unroll
-        for (int i = 0; i < NB * ATOM / 16 / 128; ++i) {
-          uint4 v = xb[i * 128 + tid];
+        for (int i = 0; i < NB * ATOM / 16 / CT; ++i) {
+          uint4 v = xb[i * CT + tid];
           v.x = h2_to_bf2(v.x); v.y = h2_to_bf2(v.y); v.z = h2_to_bf2(v.z); v.w = h2_to_bf2(v.w);
-          xb[i * 128 + tid] = v;
+          xb[i * CT + tid] = v;
         }
         fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&bars->conv[st]));
-        if (++st == STAGES) { st = 0; ph ^= 1; }
+        bar_sync(1, CT);
       }
+      const uint32_t a_addr = smem0 + st * STAGE_BYTES;
+      const uint64_t da = make_desc_mn_sw128(a_addr + wg * ATOM, ATOM), db = make_desc_mn_sw128(a_addr + 2 * ATOM, ATOM);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < KP / 16; ++k)  // 16 pixels = 2048 B further along K
+        wgmma_ss<BN, true>(d, da + static_cast<uint64_t>(k * 128), db + static_cast<uint64_t>(k * 128),
+                           (it | k) != 0 ? 1 : 0, 1);
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(smem_u32(&bars->empty[st]));
+      if (++st == STAGES) { st = 0; ph ^= 1; }
     }
+    const float* tile = stage_acc<BN>(d, smem_gen);
     // ------------------------------------------------------------------ epilogue
-    const int n = n0 + tid;  // accumulator row == output channel
-    const uint32_t lane_sel = static_cast<uint32_t>(warp * 32) << 16;
-    mbar_wait(smem_u32(&bars->acc_full), 0);
-    tc_fence_after();
-    float* wrow = p.ws + (static_cast<size_t>(g) * p.Cout + n) * p.Cin_s;
-    const bool plain = p.splits == 1;
+    if (warp < 4) {
+      const int n = n0 + tid;  // accumulator row == output channel
+      float* wrow = p.ws + split * p.ws_size + (static_cast<size_t>(g) * p.Cout + n) * p.Cin_s;
 #pragma unroll 1
-    for (int cc = 0; cc < BN / 32; ++cc) {
-      const int cb = c0 + cc * 32;
-      if (cb >= p.Cin) break;
-      uint32_t v[32];
-      tmem_ld32(tmem + lane_sel + cc * 32, v);
-      tmem_wait_ld();
-      if (n < p.Cout) {
-        if (cb + 32 <= p.Cin_s) {
-          float* dst = wrow + cb;
+      for (int cc = 0; cc < BN / 32; ++cc) {
+        const int cb = c0 + cc * 32;
+        if (cb >= p.Cin) break;
+        uint32_t v[32];
+        acc_ld32(tile + tid * (BN + 4) + cc * 32, v);
+        if (n < p.Cout) {
+          if (cb + 32 <= p.Cin_s) {
+            float* dst = wrow + cb;
 #pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            const float a = __uint_as_float(v[4 * q]), b = __uint_as_float(v[4 * q + 1]),
-                        c = __uint_as_float(v[4 * q + 2]), d = __uint_as_float(v[4 * q + 3]);
-            if (plain) *reinterpret_cast<float4*>(dst + 4 * q) = make_float4(a, b, c, d);
-            else red_add_v4(dst + 4 * q, a, b, c, d);
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (cb + i < p.Cin_s) {
-              if (plain) wrow[cb + i] = __uint_as_float(v[i]);
-              else atomicAdd(wrow + cb + i, __uint_as_float(v[i]));
+            for (int q = 0; q < 8; ++q) {
+              const float a = __uint_as_float(v[4 * q]), b = __uint_as_float(v[4 * q + 1]),
+                          c = __uint_as_float(v[4 * q + 2]), d = __uint_as_float(v[4 * q + 3]);
+              *reinterpret_cast<float4*>(dst + 4 * q) = make_float4(a, b, c, d);
             }
+          } else {
+#pragma unroll
+            for (int i = 0; i < 32; ++i)
+              if (cb + i < p.Cin_s) wrow[cb + i] = __uint_as_float(v[i]);
+          }
         }
       }
     }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc(tmem, BN);
   }
 }
 
 }  // namespace
 
-int tapwgrad_launch(const cocos_tapwgrad_desc* d, cudaStream_t stream) {
+int tapwgrad_launch(const cocos_tapwgrad_desc* d, long long* need_out, cudaStream_t stream) {
   if (!d || !d->dy || !d->x || !d->ws) {
     set_error("tapwgrad: null pointer argument");
     return -1;
@@ -284,14 +233,27 @@ int tapwgrad_launch(const cocos_tapwgrad_desc* d, cudaStream_t stream) {
   const int BN = d->Cin > 128 ? 256 : 128;
   const int mt = (d->Cout + BM - 1) / BM, nt = (d->Cin + BN - 1) / BN;
   // split-K: ~2 waves of CTAs, at least 8 chunks (512 pixels) per CTA so prologue / epilogue amortise
-  int splits = (2 * 148 + mt * nt * d->ngroups - 1) / (mt * nt * d->ngroups);
+  int splits = (2 * num_sms() + mt * nt * d->ngroups - 1) / (mt * nt * d->ngroups);
   const int max_splits = (p.total_chunks + 7) / 8;
   if (splits > max_splits) splits = max_splits;
   if (splits < 1) splits = 1;
   p.chunks_per_split = (p.total_chunks + splits - 1) / splits;
   p.splits = (p.total_chunks + p.chunks_per_split - 1) / p.chunks_per_split;
-  if (p.splits > 1)
-    COCOS_CUDA_CHECK(cudaMemsetAsync(d->ws, 0, sizeof(float) * (size_t)d->ngroups * d->Cout * d->Cin_s, stream));
+  p.ws_size = (long long)d->ngroups * d->Cout * d->Cin_s;
+  const long long need = p.splits > 1 ? p.splits * p.ws_size : 0;
+  if (need_out) {  // size query: nothing is launched
+    *need_out = need;
+    return 0;
+  }
+  if (need > 0 && (!d->part || d->part_floats < need)) {
+    set_error("tapwgrad: split-K workspace of %lld floats, %lld needed", d->part ? d->part_floats : 0ll, need);
+    return -1;
+  }
+  if (p.splits > 1) {
+    // slices are zeroed like ws would be: a tile does not store the channels of a row past its last 32-channel run
+    p.ws = d->part;
+    COCOS_CUDA_CHECK(cudaMemsetAsync(p.ws, 0, sizeof(float) * p.splits * p.ws_size, stream));
+  }
 
   CUtensorMap tm_dy, tm_x;
   int rc;
@@ -320,6 +282,7 @@ int tapwgrad_launch(const cocos_tapwgrad_desc* d, cudaStream_t stream) {
     tapwgrad_kernel<128><<<grid, NUM_THREADS, smem_bytes, stream>>>(tm_dy, tm_x, p);
   }
   COCOS_CUDA_CHECK(cudaGetLastError());
+  if (p.splits > 1) return ordered_sum(p.ws, p.splits, p.ws_size, d->ws, 0, stream);
   return 0;
 }
 

@@ -17,6 +17,77 @@ void set_error(const char* fmt, ...) {
 }
 const char* get_error() { return g_err; }
 
+int workspace_check(float* ws, long long* ws_floats, long long need, const char* what) {
+  if (!ws_floats) {
+    set_error("%s: null workspace size pointer", what);
+    return -1;
+  }
+  if (!ws) {
+    *ws_floats = need;
+    return 1;
+  }
+  if (*ws_floats < need) {
+    set_error("%s: workspace of %lld floats, %lld needed", what, *ws_floats, need);
+    return -1;
+  }
+  return 0;
+}
+
+int num_sms() {
+  static int n = 0;
+  if (n == 0) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        n <= 0)
+      n = 132;
+  }
+  return n;
+}
+
+namespace {
+// few partials per output (split-K slices): one thread per output adds them in order
+__global__ void __launch_bounds__(256)
+ordered_sum_kernel(const float* __restrict__ part, int nparts, long long n, float* __restrict__ out, int accumulate) {
+  for (long long i = blockIdx.x * 256ll + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * 256) {
+    float t = 0.f;
+    for (int p = 0; p < nparts; ++p) t += part[p * n + i];
+    out[i] = accumulate ? out[i] + t : t;
+  }
+}
+// many partials per output (per-block statistics, losses): one block per output, thread k adds partials k, k + 256, ...
+// and a fixed tree combines the 256 sums
+__global__ void __launch_bounds__(256)
+ordered_sum_wide_kernel(const float* __restrict__ part, int nparts, long long n, float* __restrict__ out,
+                        int accumulate) {
+  __shared__ float red[256];
+  for (long long i = blockIdx.x; i < n; i += gridDim.x) {
+    float t = 0.f;
+    for (int p = threadIdx.x; p < nparts; p += 256) t += part[p * n + i];
+    red[threadIdx.x] = t;
+    __syncthreads();
+    for (int w = 128; w > 0; w >>= 1) {
+      if (threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) out[i] = accumulate ? out[i] + red[0] : red[0];
+    __syncthreads();
+  }
+}
+}  // namespace
+
+int ordered_sum(const float* part, int nparts, long long n, float* out, int accumulate, cudaStream_t stream) {
+  if (nparts > 32) {
+    const long long blocks = n < num_sms() * 8ll ? n : num_sms() * 8ll;
+    ordered_sum_wide_kernel<<<static_cast<int>(blocks), 256, 0, stream>>>(part, nparts, n, out, accumulate);
+  } else {
+    long long blocks = (n + 255) / 256;
+    if (blocks > num_sms() * 8ll) blocks = num_sms() * 8ll;
+    ordered_sum_kernel<<<static_cast<int>(blocks), 256, 0, stream>>>(part, nparts, n, out, accumulate);
+  }
+  COCOS_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);

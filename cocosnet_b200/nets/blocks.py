@@ -3,7 +3,7 @@
 checkpoints load: reference models/networks/normalization.py,
 architecture.py).  The attention matrix product, the SPADE modulation, the
 instance-norm/activation pairs and the FORWARD of every stride-1 3x3 / 1x1
-convolution run on hand-written sm_100a kernels; conv backward (dgrad/wgrad) and
+convolution run on hand-written sm_90a kernels; conv backward (dgrad/wgrad) and
 the strided 4x4 convolutions still go through cuDNN.
 """
 import re
@@ -24,7 +24,7 @@ class strict_convs:
     """Context for the layers that have no kernel on the NHWC pipeline yet (SPADE with batch / instance statistics:
     the celebahq / deepfashion configs) when the 1e-3 parity mode is on (--conv_precision split): their convolutions
     run in plain fp32 (cuDNN, TF32 off) instead of single-term fp16 / TF32, whose rounding the correlation's
-    1/temperature = 100 amplifies to 5e-3 on warp_out (profiles/r02_parity_*.txt)."""
+    1/temperature = 100 amplifies to several 1e-3 on warp_out."""
 
     def __init__(self, on=True):
         self.on = on
@@ -46,7 +46,7 @@ class strict_convs:
 
 def conv_apply(conv, x):
     """`conv(x)` for an nn.Conv2d (possibly wrapped by spectral_norm / equal_lr): stride-1 3x3 / 1x1 convolutions
-    run their forward on the tcgen05 implicit-GEMM kernel (K2, fp16 operands / fp32 accumulate, TF32-class
+    run their forward on the wgmma implicit-GEMM kernel (K2, fp16 operands / fp32 accumulate, TF32-class
     precision); anything else, or `COCOS_NATIVE_CONV=0`, falls back to the module (cuDNN)."""
     if (_ops.NATIVE_CONV and not _ops.STOCK_TORCH and not _STRICT[0] and isinstance(conv, nn.Conv2d) and x.is_cuda and x.dtype == torch.float32
             and conv.stride == (1, 1) and conv.dilation == (1, 1) and conv.groups == 1
@@ -155,7 +155,7 @@ def nonspade_norm(opt, norm_type="instance"):
 def norm_act(layer, x, slope=None):
     """leaky_relu(layer(x), slope) for a `nonspade_norm` product (a conv, or Sequential(conv, norm));
     slope None = no activation.  conv -> InstanceNorm2d(affine=False) -> LeakyReLU runs as the conv plus ONE
-    fused sm_100a kernel (forward and backward) instead of stats / normalise / activation passes."""
+    fused sm_90a kernel (forward and backward) instead of stats / normalise / activation passes."""
     if isinstance(layer, nn.Sequential) and len(layer) == 2 and isinstance(layer[1], nn.InstanceNorm2d) \
             and not layer[1].affine and not layer[1].track_running_stats:
         y = conv_apply(layer[0], x)
@@ -214,7 +214,7 @@ class SPADE(nn.Module):
         """norm(x) * (1 + gamma) + beta [-> leaky_relu] [-> reflection pad]."""
         gb = self.gamma_beta(x, segmap)
         if self.pono and x.is_cuda and x.dtype == torch.float32 and not _ops.STOCK_TORCH:
-            # PONO + modulation + activation + reflection pad: one fused sm_100a kernel each way
+            # PONO + modulation + activation + reflection pad: one fused sm_90a kernel each way
             return _ops.spade_mod(x, gb, pad=pad, slope=1.0 if leaky is None else leaky)
         gamma, beta = gb.chunk(2, dim=1)
         out = self.param_free_norm(x) * (1 + gamma) + beta

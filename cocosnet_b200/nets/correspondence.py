@@ -2,7 +2,7 @@
 models/networks/correspondence.py:13-36, 79-146, 148-374).
 
 The dense N x N part of forward (correspondence.py:272-372) is
-cocosnet_b200.corr.correspondence_tail: one fused sm_100a kernel per softmax
+cocosnet_b200.corr.correspondence_tail: one fused sm_90a kernel per softmax
 direction, nothing N x N in HBM.
 """
 import torch

@@ -1,7 +1,7 @@
 """Network forwards on the 16-bit NHWC tape (cocosnet_b200/tape.py): the SPADE generator, the domain adaptors, the
 residual-block stack with the theta / phi convolutions, the PatchGAN discriminators and the VGG19 feature net of the
 reference (models/networks/generator.py:60-89,140-160; architecture.py:70-95; normalization.py:129-151;
-correspondence.py:13-36,108-146,260-272; discriminator.py:138-177) as chains of hand-written sm_100a kernels: every
+correspondence.py:13-36,108-146,260-272; discriminator.py:138-177) as chains of hand-written sm_90a kernels: every
 convolution (forward, backward-data, backward-weights) on the tap-convolution kernels, every normalisation /
 modulation / activation / padding step on the NHWC elementwise kernels, activations fp16 (fp32 + 2-term split
 operands on the path that feeds the correlation), gradients bf16.

@@ -40,7 +40,7 @@ class SPADEGenerator(BaseNetwork):
 
     def forward(self, input, warp_out=None):
         seg = input if warp_out is None else warp_out
-        if _fast.generator_supported(self, seg):  # 16-bit NHWC pipeline, every conv / norm on sm_100a kernels
+        if _fast.generator_supported(self, seg):  # 16-bit NHWC pipeline, every conv / norm on sm_90a kernels
             return _fast.generator_forward(self, seg)
         with strict_convs(seg.is_cuda and _fast.conv_precision(self.opt) == "split"):
             return self._forward_modules(seg)

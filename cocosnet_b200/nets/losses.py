@@ -45,7 +45,7 @@ class GANLoss(nn.Module):
 
 class _CtxRows(torch.autograd.Function):
     """cx[b,i] = max_j A_ij from the normalised features: the N x N part of the contextual loss on hand-written
-    kernels -- S = Xhat^T Yhat on the tcgen05 GEMM (3-term split fp16 operands: the loss divides by min_j (1 - S)),
+    kernels -- S = Xhat^T Yhat on the wgmma GEMM (3-term split fp16 operands: the loss divides by min_j (1 - S)),
     one warp per row for min / exp / sum, and in the backward dS (bf16) + one more GEMM for dXhat.  The reference keeps
     d, d_norm, w, A ([B,N,N] fp32 each) and their autograd copies."""
 

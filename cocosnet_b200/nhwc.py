@@ -2,7 +2,7 @@
 C-ABI (include/cocos_b200.h: cocos_tapconv, cocos_tapwgrad, cocos_pack_w, cocos_spade_mod_nhwc_*,
 cocos_inst_act_nhwc_*, cocos_nhwc_pack / unpack, cocos_colsum_nhwc).
 
-Everything here is layout / planning logic; the arithmetic runs in the sm_100a kernels.  `BACKEND` is the object
+Everything here is layout / planning logic; the arithmetic runs in the sm_90a kernels.  `BACKEND` is the object
 that enqueues kernels: the native one (ctypes -> libcocos_b200.so) is the only one the product ever uses and it
 raises when the library is missing.  The CPU tests install a torch emulation of the same entry points
 (oracle/nhwc_emul.py) to check the planning logic against F.conv2d / autograd without a GPU.
@@ -113,7 +113,8 @@ class _TapwgradDesc(ctypes.Structure):
     _fields_ = [("dy", ctypes.c_void_p), ("x", ctypes.c_void_p), ("ws", ctypes.c_void_p)] + \
                [(n, ctypes.c_int) for n in ("B", "H", "W", "dy_Cs", "Cout", "Hin", "Win", "Ca", "a_stride", "x_f16",
                                             "Cin", "Cin_s", "ngroups")] + \
-               [("dh", ctypes.c_byte * MAXG), ("dw", ctypes.c_byte * MAXG), ("coff", ctypes.c_short * MAXG)]
+               [("dh", ctypes.c_byte * MAXG), ("dw", ctypes.c_byte * MAXG), ("coff", ctypes.c_short * MAXG),
+                ("part", ctypes.c_void_p), ("part_floats", ctypes.c_longlong)]
 
 
 def _stream():
@@ -173,6 +174,11 @@ class NativeBackend:
         desc.ngroups = len(groups)
         for i, g in enumerate(groups):
             desc.dh[i], desc.dw[i], desc.coff[i] = g.dh, g.dw, g.coff
+        need = ctypes.c_longlong(0)
+        _lib.check(self.lib.cocos_tapwgrad_workspace(ctypes.byref(desc), ctypes.byref(need)), "cocos_tapwgrad_workspace",
+                   kernels=0)
+        part = torch.empty((max(need.value, 1),), dtype=torch.float32, device=dy.device)  # split-K slices
+        desc.part, desc.part_floats = part.data_ptr(), part.numel()
         _lib.check(self.lib.cocos_tapwgrad(ctypes.byref(desc), _stream()), "cocos_tapwgrad")
 
     def pack_w(self, w, dst, rows, rows_alloc, kc, groups, transposed, bf16):
@@ -214,7 +220,7 @@ class NativeBackend:
             tab = NativeBackend._sn_tables[key] = (table, ba, bb, snap, offs)
         table, ba, bb, snap, offs = tab
         n = len(entries)
-        scratch = torch.empty((2 * n,), dtype=torch.float32, device=dev)
+        scratch = torch.empty((2 * n + ba + bb,), dtype=torch.float32, device=dev)  # per-layer sums, per-block partials
         inv = torch.empty((n,), dtype=torch.float32, device=dev)
         shot = torch.empty((snap,), dtype=torch.float32, device=dev)
         _lib.check(self.lib.cocos_sn_power_iter(table.data_ptr(), n, ba, bb, scratch.data_ptr(), inv.data_ptr(),
@@ -234,8 +240,9 @@ class NativeBackend:
                    "cocos_spade_mod_nhwc_bwd")
 
     def in_stats(self, x, stats, C):
-        _lib.check(self.lib.cocos_in_stats_nhwc(x.t.data_ptr(), x.kind, x.Cs, x.B, C, x.H * x.W, stats.data_ptr(),
-                                                _stream()), "cocos_in_stats_nhwc", kernels=2)
+        _lib.call_with_workspace(self.lib.cocos_in_stats_nhwc, (x.t.data_ptr(), x.kind, x.Cs, x.B, C, x.H * x.W,
+                                                                stats.data_ptr()), _stream(), "cocos_in_stats_nhwc",
+                                 kernels=2)
 
     def inst_fwd(self, x, stats, res, slope_ptr, slope, y, y2, eps, C, gb=None, batch_stats=False):
         _lib.check(self.lib.cocos_inst_act_nhwc_fwd(
@@ -247,13 +254,13 @@ class NativeBackend:
 
     def inst_bwd(self, dy, dy2, x, stats, res, slope_ptr, slope, bstats, dslope, dx, dx_acc, dres, dres_acc, eps, C,
                  gb=None, dgb=None, batch_stats=False, const_stats=False, phase=0):
-        _lib.check(self.lib.cocos_inst_act_nhwc_bwd(
+        _lib.call_with_workspace(self.lib.cocos_inst_act_nhwc_bwd, (
             dy.t.data_ptr(), dy.Cs, dy.pad, _p(dy2.t if dy2 else None), dy2.Cs if dy2 else 0, x.t.data_ptr(), x.kind,
             x.Cs, stats.data_ptr(), _p(res.t if res else None), res.kind if res else 0, res.Cs if res else 0,
             _p(slope_ptr), float(slope), bstats.data_ptr(), _p(dslope), dx.t.data_ptr(), dx.Cs, int(dx_acc),
             _p(dres.t if dres else None), dres.Cs if dres else 0, int(dres_acc), x.B, C, x.H, x.W, float(eps),
             _p(gb.t if gb else None), gb.kind if gb else 0, gb.Cs if gb else 0, _p(dgb.t if dgb else None),
-            dgb.Cs if dgb else 0, int(batch_stats), int(const_stats), int(phase), _stream()),
+            dgb.Cs if dgb else 0, int(batch_stats), int(const_stats), int(phase)), _stream(),
             "cocos_inst_act_nhwc_bwd", kernels=3 if phase == 0 else (2 if phase == 1 else 1))
 
     def act_bwd(self, dy, y, dz, C, act, slope):
@@ -267,9 +274,10 @@ class NativeBackend:
                                             hs, ws, dst.H, dst.W, f, dst.pad, _stream()), "cocos_nhwc_pack")
 
     def pair_loss_fwd(self, x, y, w, scale, mode, out):
-        _lib.check(self.lib.cocos_pair_loss_nhwc_fwd(x.t.data_ptr(), x.Cs, y.t.data_ptr(), y.Cs, _p(w), x.B, x.H * x.W,
-                                                     x.C, float(scale), int(mode), out.data_ptr(), _stream()),
-                   "cocos_pair_loss_nhwc_fwd")
+        _lib.call_with_workspace(self.lib.cocos_pair_loss_nhwc_fwd, (x.t.data_ptr(), x.Cs, y.t.data_ptr(), y.Cs, _p(w),
+                                                                     x.B, x.H * x.W, x.C, float(scale), int(mode),
+                                                                     out.data_ptr()), _stream(),
+                                 "cocos_pair_loss_nhwc_fwd", kernels=2)
 
     def pair_loss_bwd(self, x, y, w, scale, mode, g, dx, acc):
         _lib.check(self.lib.cocos_pair_loss_nhwc_bwd(x.t.data_ptr(), x.Cs, y.t.data_ptr(), y.Cs, _p(w), x.B, x.H * x.W,
@@ -295,8 +303,8 @@ class NativeBackend:
                                               int(acc), _stream()), "cocos_nhwc_unpack")
 
     def colsum(self, x2d, kind, Cs, C, rows, out):
-        _lib.check(self.lib.cocos_colsum_nhwc(x2d.data_ptr(), kind, Cs, C, rows, out.data_ptr(), _stream()),
-                   "cocos_colsum_nhwc", kernels=2)
+        _lib.call_with_workspace(self.lib.cocos_colsum_nhwc, (x2d.data_ptr(), kind, Cs, C, rows, out.data_ptr()),
+                                 _stream(), "cocos_colsum_nhwc", kernels=2)
 
 
 _BACKEND = None

@@ -1,7 +1,7 @@
 """torch-tensor wrappers over the C-ABI (device pointers + current stream).
 
 PyTorch is plumbing here: it owns device memory and the stream; all math on
-the hot path runs in the hand-written sm_100a kernels of csrc/.
+the hot path runs in the hand-written sm_90a kernels of csrc/.
 """
 import torch
 
@@ -10,10 +10,10 @@ from . import _lib
 
 import os as _os
 
-# forward of stride-1 3x3 / 1x1 convolutions on the tcgen05 implicit-GEMM kernel (COCOS_NATIVE_CONV=0: cuDNN)
+# forward of stride-1 3x3 / 1x1 convolutions on the wgmma implicit-GEMM kernel (COCOS_NATIVE_CONV=0: cuDNN)
 NATIVE_CONV = _os.environ.get("COCOS_NATIVE_CONV", "1") != "0"
 # MEASUREMENT ONLY (bench.py's gpu_baseline leg): every hand-written kernel off, the mirror modules run the reference's
-# own torch expressions on cuDNN / cuBLAS -- "stock PyTorch on the same B200", the bar SURVEY.md 8d names.
+# own torch expressions on cuDNN / cuBLAS -- "stock PyTorch on the same GPU", the bar SURVEY.md 8d names.
 STOCK_TORCH = _os.environ.get("COCOS_STOCK_TORCH", "0") == "1"
 
 
@@ -308,7 +308,7 @@ def _conv_kernel(x16, wt, bias, b, h, w, hin, win, cp, cout, ks, off):
 
 def conv_fwd_native(x, weight, bias, pre_padded):
     """K2 forward.  x fp32 NCHW [B,Cin,Hin,Win] (pre_padded: Hin = H + KS - 1), weight [Cout,Cin,KS,KS] -> y fp32
-    NCHW [B,Cout,H,W] on the tcgen05 implicit-GEMM kernel (fp16 operands, fp32 accumulate)."""
+    NCHW [B,Cout,H,W] on the wgmma implicit-GEMM kernel (fp16 operands, fp32 accumulate)."""
     x = x.contiguous()
     _req(x, torch.float32, "x")
     b, cin, hin, win = x.shape
@@ -354,7 +354,7 @@ WGRAD_X_BF16 = _os.environ.get("COCOS_WGRAD_X_BF16", "1") == "1"  # mixed bf16 x
 
 def conv_wgrad_native(dy, x, ks, pre_padded):
     """K2w backward-weights (NCHW operands, the fallback path of layers that are not on the NHWC tape): dW
-    [Cout,Cin,KS,KS] = sum over pixels of dy x shifted x (bf16 operands, fp32 accumulate) on the split-K tcgen05 kernel.
+    [Cout,Cin,KS,KS] = sum over pixels of dy x shifted x (bf16 operands, fp32 accumulate) on the split-K wgmma kernel.
     dy [B,Cout,H,W], x [B,Cin,Hin,Win] fp32 NCHW, W >= 64."""
     b, cout, h, w = dy.shape
     _, cin, hin, win = x.shape
@@ -362,21 +362,21 @@ def conv_wgrad_native(dy, x, ks, pre_padded):
     dy16 = cast_pitch(dy, True)
     x16 = cast_pitch(x, WGRAD_X_BF16, wout=w, nshift=ks, off=off)
     ws = torch.empty((ks * ks, cin, cout), dtype=torch.float32, device=dy.device)
-    _lib.check(_lib.lib().cocos_conv_wgrad(dy16.data_ptr(), x16.data_ptr(), ws.data_ptr(), b, h, w, hin, win, cout, cin,
-                                           ks, off, 1, int(WGRAD_X_BF16), _stream()),
-               "cocos_conv_wgrad")
+    _lib.call_with_workspace(_lib.lib().cocos_conv_wgrad, (dy16.data_ptr(), x16.data_ptr(), ws.data_ptr(), b, h, w, hin,
+                                                           win, cout, cin, ks, off, 1, int(WGRAD_X_BF16)), _stream(),
+                             "cocos_conv_wgrad")
     return ws.view(ks, ks, cin, cout).permute(3, 2, 0, 1).contiguous()
 
 
 NATIVE_WGRAD = _os.environ.get("COCOS_NATIVE_WGRAD", "1") == "1"
-# backward-data on K2 costs one more transpose-pack + weight re-layout per layer: measured on the eager ade20k step
-# (launch-bound, profiles/README.md) 179 ms with it vs 170.5 ms without, although the GPU-busy time is lower with it
-# (160 vs 163 ms) -- so Pix2PixTrainer turns it on exactly when the iteration is replayed from a CUDA graph.
+# backward-data on K2 costs one more transpose-pack + weight re-layout per layer: it lowers the GPU-busy time but adds
+# launches to the launch-bound eager step -- so Pix2PixTrainer turns it on exactly when the iteration is replayed from
+# a CUDA graph.
 NATIVE_DGRAD = _os.environ.get("COCOS_NATIVE_DGRAD", "0") == "1"
 
 
 class _ConvNative(torch.autograd.Function):
-    """conv2d (stride 1, KS in {1,3}): forward, backward-data and backward-weights on the tcgen05 implicit-GEMM
+    """conv2d (stride 1, KS in {1,3}): forward, backward-data and backward-weights on the wgmma implicit-GEMM
     kernels (conv.cu, conv_wgrad.cu); COCOS_NATIVE_WGRAD=0 sends the weight gradient through cuDNN instead."""
 
     @staticmethod

@@ -76,7 +76,7 @@ _BASE = [
     ("--mask_noise", dict(action="store_true")),
     ("--noise_for_mask", dict(action="store_true")),
     ("--video_like", dict(action="store_true")),
-    # --- B200 build only (not in the reference) ---
+    # --- native build only (not in the reference) ---
     ("--corr_precision", dict(type=str, default="auto", choices=("auto", "fp16", "split"))),
     ("--conv_precision", dict(type=str, default="split", choices=("split", "mixed", "fast"))),
     ("--channels_last", dict(action="store_true")),

@@ -8,7 +8,7 @@ grads on the D step) and divided by the world size -- the reference's
 `sum(losses).mean()` over replicas.  No per-step parameter broadcast.
 
 `run_step` is the launch-bound answer for one GPU: the whole G+D iteration (both forwards, both backwards, both
-fused-Adam updates: ~12 000 kernel launches, which the Python/ATen dispatcher cannot issue as fast as a B200 retires
+fused-Adam updates: ~12 000 kernel launches, which the Python/ATen dispatcher cannot issue as fast as an H100 retires
 them) is captured ONCE into a CUDA graph after a few eager iterations and replayed from static input buffers.
 """
 import os
@@ -94,7 +94,7 @@ class Pix2PixTrainer:
         self.pix2pix_model = Pix2PixModel(opt)
         if len(opt.gpu_ids) > 0:
             self.pix2pix_model.cuda()
-            # fixed shapes every step: let cuDNN pick its fastest algorithms (measured -5 % step time on B200)
+            # fixed shapes every step: let cuDNN pick its fastest algorithms
             torch.backends.cudnn.benchmark = not getattr(opt, "no_cudnn_benchmark", False)
             if getattr(opt, "channels_last", False):  # NHWC activations: no cuDNN layout transposes
                 self.pix2pix_model.to(memory_format=torch.channels_last)
@@ -128,7 +128,7 @@ class Pix2PixTrainer:
         self.pre_sharded = bool(getattr(opt, "pre_sharded", False))
         if opt.isTrain and "COCOS_NATIVE_DGRAD" not in os.environ:
             # K2 backward-data lowers the GPU-busy time but adds launches: it pays off once the iteration is replayed
-            # from a graph and costs 5 % on the launch-bound eager step (profiles/README.md, r01 A/B)
+            # from a graph and costs time on the launch-bound eager step
             from . import ops
             ops.NATIVE_DGRAD = self.graph_capable()
 

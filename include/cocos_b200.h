@@ -1,4 +1,4 @@
-/* cocos_b200 — C-ABI of the B200-native CoCosNet hot path (libcocos_b200.so).
+/* cocos_b200 — C-ABI of the H100-native CoCosNet hot path (libcocos_b200.so).
  *
  * The reference (microsoft/CoCosNet) has no native boundary: its hot path is
  * Python calling ATen.  This header is the boundary we put underneath the
@@ -20,7 +20,14 @@
 extern "C" {
 #endif
 
-#define COCOS_ABI_VERSION 6
+#define COCOS_ABI_VERSION 7
+
+/* Multi-block reductions (cocos_conv_wgrad, cocos_tapwgrad, cocos_sn_power_iter, cocos_in_stats_nhwc,
+ * cocos_inst_act_nhwc_bwd, cocos_pair_loss_nhwc_fwd, cocos_colsum_nhwc) write one partial sum per block into a
+ * caller-provided fp32 workspace and add the partials in a fixed order: the same inputs give the same bits on every
+ * run.  Workspace arguments (ws, ws_floats): ws == NULL is a size query -- *ws_floats receives the floats needed and
+ * nothing is launched; otherwise *ws_floats is the capacity of ws.  The workspace must stay untouched until the work
+ * enqueued on `stream` has finished. */
 
 int cocos_abi_version(void);
 const char* cocos_last_error(void);
@@ -61,7 +68,7 @@ int cocos_corr_warp_fwd(const void* q, const void* k, const void* vt, const floa
                         float* corr, int B, int Nq, int Nk, int Kd, int Cv, int Cvp, int Nkp, float scale,
                         void* stream);
 
-/* Batched tcgen05 GEMM: C[b] (MxN fp32 row-major, ldc) = alpha * A[b] (MxK fp16,
+/* Batched wgmma GEMM: C[b] (MxN fp32 row-major, ldc) = alpha * A[b] (MxK fp16,
  * K contiguous, lda) * B[b]^T (NxK fp16, ldb) (+ C[b] if accumulate); `bf16` != 0
  * treats both operands as bf16.  Strides in
  * elements.  The torch.matmul / 1x1-conv call sites of correspondence.py:291
@@ -97,7 +104,7 @@ int cocos_spade_mod_bwd(const float* dy, const float* x, const float* gb, const 
                         float* dx, float* dgb, int B, int C, int H, int W, int pad, float slope, int nhwc,
                         void* stream);
 
-/* K2: TMA-fed tcgen05 implicit-GEMM convolution, forward, KS in {1, 3}, stride 1 (the 3x3 convs of the SPADE blocks,
+/* K2: TMA-fed wgmma implicit-GEMM convolution, forward, KS in {1, 3}, stride 1 (the 3x3 convs of the SPADE blocks,
  * domain adaptor and residual blocks: architecture.py:31-33,73-74; normalization.py:112-120; correspondence.py:17-22).
  *   y[b,n,h,w] = bias[n] + sum_{r,s,c} x[b, h + r - off, w + s - off, c] * wt[n, (r*KS + s)*Cp + c]
  * x  : fp16 (bf16 if `bf16`) NHWC [B, Hin, Win, Cp], Cp % 64 == 0 (cocos_pack_rows_f16 of the NCHW tensor viewed as
@@ -115,7 +122,7 @@ int cocos_conv_fwd(const void* x, const void* wt, const float* bias, float* y, i
 int cocos_cast_pitch(const float* src, void* dst, long long rows, int Win, int Wout, int Wp, int nshift, int off,
                      int bf16, void* stream);
 
-/* K2w: convolution backward-weights (stride 1, KS in {1,3}) as a tcgen05 GEMM over the B*H*W pixels, split-K over the
+/* K2w: convolution backward-weights (stride 1, KS in {1,3}) as a wgmma GEMM over the B*H*W pixels, split-K over the
  * grid.  Replaces the wgrad half of autograd's convolution_backward for the same nn.Conv2d call sites as
  * cocos_conv_fwd.
  *   ws[(r*KS + s), c, n] = sum_{b,h,w} dy[b, n, h, w] * x[b, c, h + r - off, w + s - off]
@@ -124,9 +131,9 @@ int cocos_cast_pitch(const float* src, void* dst, long long rows, int Win, int W
  *      rows outside [0,Hin) are zero.  off = 0 when x carries its halo, KS/2 for zero padding.
  * W >= 64 only (narrower layers: error return; the host mirror sends them to the library wgrad); both operands bf16
  * (dy_bf16 = x_bf16 = 1): a bf16 x fp16 instruction descriptor is rejected by the hardware.
- * ws : fp32 [KS*KS, Cin, Cout], fully overwritten (zeroed + atomically accumulated when the pixel range is split). */
+ * ws : fp32 [KS*KS, Cin, Cout], fully overwritten (split-K partials are added in split order: the same bits on every run). */
 int cocos_conv_wgrad(const void* dy, const void* x, float* ws, int B, int H, int W, int Hin, int Win, int Cout, int Cin,
-                     int KS, int off, int dy_bf16, int x_bf16, void* stream);
+                     int KS, int off, int dy_bf16, int x_bf16, float* part, long long* part_floats, void* stream);
 
 /* Fused operand prologue for `--PONO_C` (correspondence.py:273-281 / 283-289): x fp32 [B,C,h,w] (output of the theta
  * or phi 1x1 conv) -> unfold(match_kernel, zero pad) -> minus the mean over K = C*mk*mk -> / (L2 norm over K + eps)
@@ -156,7 +163,7 @@ int cocos_inst_act_bwd(const float* dy, const float* x, const float* mean, const
 
 /* ------------------------------------------------------------------------------------------------------------------
  * 16-bit NHWC pipeline (round 2): every convolution of the generator / adaptor / residual blocks / PatchGAN / VGG19 is
- * ONE persistent tcgen05 kernel over NHWC activations, described by a list of "tap groups"; the kernels between two
+ * ONE wgmma kernel over NHWC activations, described by a list of "tap groups"; the kernels between two
  * convolutions (normalisation, modulation, activation, halo) read and write the same 16-bit NHWC tensors, so an
  * activation crosses HBM once per producer / consumer instead of as fp32 NCHW + transposes + re-packs.
  * Tensor kinds: 1 = fp16, 2 = bf16, 3 = fp32 (all NHWC [B, H, W, Cs], channel stride Cs >= C); 0 = fp32 NCHW.
@@ -217,7 +224,9 @@ int cocos_tapconv(const cocos_tapconv_desc* desc, void* stream);
  * (the backward-weights half of convolution_backward for the layers cocos_tapconv serves).
  *   dy : bf16 NHWC [B, H, W, dy_Cs];  x: NHWC [B, Hin, Win, Ca] as the forward read it, fp16 (x_f16 = 1: converted
  *        to bf16 inside the kernel) or bf16;  ws: fp32 [ngroups, Cout, Cin_s], Cin_s >= Cin, Cin_s % 4 == 0, fully
- *        overwritten (columns >= Cin undefined). */
+ *        overwritten (columns >= Cin undefined).
+ *   part / part_floats: split-K workspace and its capacity in floats (cocos_tapwgrad_workspace gives the need; 0:
+ *        part may be NULL). */
 typedef struct cocos_tapwgrad_desc {
   const void* dy;
   const void* x;
@@ -229,8 +238,11 @@ typedef struct cocos_tapwgrad_desc {
   signed char dh[COCOS_TAPCONV_MAX_GROUPS];
   signed char dw[COCOS_TAPCONV_MAX_GROUPS];
   short coff[COCOS_TAPCONV_MAX_GROUPS];
+  float* part;
+  long long part_floats;
 } cocos_tapwgrad_desc;
 int cocos_tapwgrad(const cocos_tapwgrad_desc* desc, void* stream);
+int cocos_tapwgrad_workspace(const cocos_tapwgrad_desc* desc, long long* floats);
 
 /* Weight matrix of a tap-group list from an nn.Conv2d weight fp32 [Cout, Cin, KS, KS]:
  * dst[row, g*Kc + c] (16-bit, fp16 or bf16) for row < rows_alloc, g < ngroups, c < Kc (Kc % 64 == 0); zero for
@@ -269,7 +281,8 @@ int cocos_ctx_rows_bwd(const float* S, const float* g, void* dS, int B, int N, i
  * of the layer's [u | v] copy in `snapshot` (may be NULL; the vectors the backward of this forward needs)}.
  * training != 0: one power iteration, u and v updated in place (v <- normalize(W^T u), u <- normalize(W v)); then
  * inv_sigma[i] = 1 / (u^T W v).  The normalised weight is never formed: cocos_tapconv takes inv_sigma as `scale`.
- * scratch: 2n floats.  blocks_a / blocks_b: total blocks of the two phases. */
+ * scratch: 2n + blocks_a + blocks_b floats (per-layer |W^T u|^2 and |W v|^2, or u^T W v in evaluation, then the
+ * per-block partials).  blocks_a / blocks_b: total blocks of the two phases. */
 int cocos_sn_power_iter(const void* table, int n, int blocks_a, int blocks_b, float* scratch, float* inv_sigma,
                         float* snapshot, float eps, int training, void* stream);
 /* Per-pixel PONO statistics of x (kind 1|3) [npix, Cs] over its C channels: mean and 1/sqrt(unbiased var + eps)
@@ -279,7 +292,8 @@ int cocos_pono_stats_nhwc(const void* x, int kind, int Cs, int C, long long npix
 
 /* InstanceNorm2d(affine=False) statistics over NHWC: stats[b, c] = {sum, sum of squares} over the HW pixels
  * (generator.py:104-113, discriminator.py:92-115, correspondence.py:19,23 with normalization.py:52-53). */
-int cocos_in_stats_nhwc(const void* x, int kind, int Cs, int B, int C, int HW, float* stats, void* stream);
+int cocos_in_stats_nhwc(const void* x, int kind, int Cs, int B, int C, int HW, float* stats, float* ws,
+                        long long* ws_floats, void* stream);
 
 /* y = act( instance_norm(x) [+ res] ), act = LeakyReLU(slope) or PReLU (slope_ptr: device scalar, correspondence.py:20)
  * [, reflection halo y_pad, lo term, second fp32 copy y2 without halo].  Backward: dy bf16 (halo folded) [+ dy2] ->
@@ -293,7 +307,7 @@ int cocos_inst_act_nhwc_bwd(const void* dy, int dy_Cs, int dy_pad, const void* d
                             const float* slope_ptr, float slope, float* bstats, float* dslope, void* dx, int dx_Cs,
                             int dx_acc, void* dres, int dres_Cs, int dres_acc, int B, int C, int H, int W, float eps,
                             const void* gb, int gb_kind, int gb_Cs, void* dgb, int dgb_Cs, int batch_stats,
-                            int const_stats, int phase, void* stream);
+                            int const_stats, int phase, float* ws, long long* ws_floats, void* stream);
 /* The same two entry points serve SPADE with instance / batch statistics (normalization.py:96-104,132-149, the
  * celebahq / deepfashion configurations): gb (kind 1|3, [B,H,W,gb_Cs], gamma at channels [0,C), beta at [C,2C))
  * modulates the normalised value, z = norm(x) * (1 + gamma) + beta, and the backward also emits dgb (bf16);
@@ -319,7 +333,7 @@ int cocos_nhwc_pack(const float* src, void* dst, int kind, int B, int C, int Cs,
  * pix2pix_model.py:256), and the gradient w.r.t. x: dx (bf16, added to its content if acc) = g[0] * scale * w[b] *
  * d/dx.  The discriminator / VGG19 features are compared where they live instead of as fp32 NCHW copies. */
 int cocos_pair_loss_nhwc_fwd(const void* x, int x_Cs, const void* y, int y_Cs, const float* w, int B, long long HW, int C,
-                             float scale, int mode, float* out, void* stream);
+                             float scale, int mode, float* out, float* ws, long long* ws_floats, void* stream);
 int cocos_pair_loss_nhwc_bwd(const void* x, int x_Cs, const void* y, int y_Cs, const float* w, int B, long long HW, int C,
                              float scale, int mode, const float* g, void* dx, int dx_Cs, int acc, void* stream);
 /* fp16 operand [npix, src_Cs] (hi at channels [0, dst_Cs), optional lo term at lo_off) -> bf16 [npix, dst_Cs] =
@@ -335,7 +349,8 @@ int cocos_maxpool2_nhwc_bwd(const void* dy, const void* x, void* dx, int B, int 
 int cocos_nhwc_unpack(const void* src, int kind, int Cs, int c_lo, int C, int B, int H, int W, int pad, float* dst,
                       int Cd, int cd_lo, int Hd, int Wd, int f, int acc, void* stream);
 /* out[c] = sum over the rows of x [rows, Cs] (kind 1|2|3), c < C: the bias gradient of a convolution. */
-int cocos_colsum_nhwc(const void* x, int kind, int Cs, int C, long long rows, float* out, void* stream);
+int cocos_colsum_nhwc(const void* x, int kind, int Cs, int C, long long rows, float* out, float* ws,
+                      long long* ws_floats, void* stream);
 
 #ifdef __cplusplus
 }

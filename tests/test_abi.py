@@ -16,7 +16,7 @@ def test_header_symbols_exported():
     for name in declared:
         assert hasattr(h, name), name
     assert declared == set(_lib.SIGNATURES), (declared ^ set(_lib.SIGNATURES))
-    assert h.cocos_abi_version() == 6
+    assert h.cocos_abi_version() == 7
 
 
 def test_ctypes_signatures_match_header_arity_and_kinds():

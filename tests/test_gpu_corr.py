@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box): the CUDA path, called
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path, called
 through the C-ABI, against the numpy oracle and the committed goldens."""
 import os
 
@@ -412,7 +412,7 @@ CONV_CASES = [
 @pytest.mark.parametrize("b,cin,cout,h,w,ks,pre_padded", [(2, 64, 64, 64, 128, 3, True), (2, 32, 200, 70, 64, 1, False),
                                                          (1, 300, 130, 64, 64, 3, False)])
 def test_conv_wgrad_native_direct(b, cin, cout, h, w, ks, pre_padded):
-    """K2w (split-K tcgen05 backward-weights, bf16 operands) vs autograd in fp64, including the narrow-channel tiles
+    """K2w (split-K wgmma backward-weights, bf16 operands) vs autograd in fp64, including the narrow-channel tiles
     the model path does not route to it."""
     import torch.nn.functional as F
     from cocosnet_b200 import ops
@@ -438,7 +438,7 @@ def test_conv_wgrad_rejects_narrow_layers():
 
 @pytest.mark.parametrize("b,cin,cout,h,w,ks,pre_padded", CONV_CASES)
 def test_conv_native_forward_and_hybrid_backward(b, cin, cout, h, w, ks, pre_padded, monkeypatch):
-    """K2 forward (tcgen05 implicit GEMM, fp16 operands) vs torch conv2d in fp64; backward-data on the same kernel
+    """K2 forward (wgmma implicit GEMM, fp16 operands) vs torch conv2d in fp64; backward-data on the same kernel
     (bf16 operands: 2^-9 relative rounding on dy and W -> ~2e-3 rel-L2), weight/bias gradients through cuDNN."""
     import torch.nn.functional as F
     from cocosnet_b200 import ops
@@ -468,7 +468,7 @@ def test_conv_native_forward_and_hybrid_backward(b, cin, cout, h, w, ks, pre_pad
 
 @pytest.mark.parametrize("b,c,hw", [(2, 512, 16), (2, 256, 32)])
 def test_contextual_loss_kernels_vs_reference_expression(b, c, hw):
-    """ContextualLoss_forward on the tcgen05 GEMM + row kernels (cocos_ctx_rows_fwd / _bwd) against the reference's
+    """ContextualLoss_forward on the wgmma GEMM + row kernels (cocos_ctx_rows_fwd / _bwd) against the reference's
     expressions in fp64 (ContextualLoss.py:93-137): per-image loss and the gradient w.r.t. the source features."""
     from cocosnet_b200.nets.losses import ContextualLoss_forward
 

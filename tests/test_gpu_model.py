@@ -1,4 +1,4 @@
-"""GPU: the full model on the fused sm_100a kernels against (a) the goldens
+"""GPU: the full model on the fused sm_90a kernels against (a) the goldens
 minted from the unmodified reference and (b) the CPU port on the same weights."""
 import os
 

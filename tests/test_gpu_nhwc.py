@@ -465,3 +465,22 @@ def test_packed_weight_cache_follows_the_parameter_version():
     q = torch.nn.Parameter(torch.zeros(64, 64, 3, 3, device="cuda"))   # very likely the recycled address
     y3 = nhwc.conv(x, q, None, padding=1, out_kind=nhwc.F32, cache_w=q).t
     assert float(y3.abs().max()) == 0.0, "stale packed weights (address reuse %s)" % (q.data_ptr() == addr)
+
+
+def test_reductions_are_bit_reproducible():
+    """The multi-block reductions (split-K backward-weights, instance-norm statistics, bias column sums) add their
+    per-block partials in a fixed order: two calls on the same inputs give identical bits."""
+    g = torch.Generator().manual_seed(5)
+    x = torch.randn(2, 64, 64, 64, generator=g).cuda()
+    dy = torch.randn(2, 64, 64, 64, generator=g).cuda()
+    xp, xs = nhwc.pack(x, nhwc.F16, pad=1), nhwc.pack(x, nhwc.F16)
+    dyp = nhwc.pack(dy, nhwc.BF16)
+
+    def run():
+        db = torch.empty(64, device="cuda")
+        nhwc.backend().colsum(dyp.t, dyp.kind, dyp.Cs, 64, dyp.B * dyp.H * dyp.W, db)
+        return nhwc.conv_wgrad(dyp, xp, 3).clone(), nhwc.in_stats(xs).clone(), db
+    a, b = run(), run()
+    torch.cuda.synchronize()
+    for u, v in zip(a, b):
+        assert torch.isfinite(u).all() and torch.equal(u, v)

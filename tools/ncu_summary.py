@@ -1,6 +1,6 @@
 """`.ncu-rep` -> JSON summary of the launches it holds (one entry per kernel name: the LAST launch captured):
 duration, tensor-pipe activity, DRAM bytes / throughput, occupancy, registers.
-python tools/ncu_summary.py gpurun_out/x.ncu-rep > profiles/x_ncu_summary.json"""
+python tools/ncu_summary.py x.ncu-rep > x_ncu_summary.json"""
 import csv
 import io
 import json

@@ -58,7 +58,7 @@ def main():
     groups = {}
     def origin(name):
         if "cocos::" in name:
-            return "cocos (hand-written sm_100a)"
+            return "cocos (hand-written sm_90a)"
         if "nchwToNhwc" in name or "nhwcToNchw" in name or "tensorTransform" in name:
             return "cuDNN layout transposes"
         if name.startswith("cutlass") or "cudnn" in name or "implicit_convolve" in name or "engines_precompiled" in name \
