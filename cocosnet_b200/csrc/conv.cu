@@ -80,7 +80,7 @@ conv_fwd_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
       for (int it = 0; it < iters; ++it) {
         const int tap = it / kc_per_tap, kc = it - tap * kc_per_tap;
         const int r = tap / p.KS, s = tap - r * p.KS;
-        mbar_wait(smem_u32(&bars->empty[st]), ph ^ 1);
+        mbar_wait_quiet(smem_u32(&bars->empty[st]), ph ^ 1);
         const uint32_t full = smem_u32(&bars->full[st]);
         mbar_expect_tx(full, a_bytes + (BN / 128) * ATOM_BYTES);
         tma_load_4d(smem0 + st * STAGE_BYTES, &tm_x, full, kc * BK, w0 + s - p.off, h0 + r - p.off, b);

@@ -92,7 +92,7 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tm_dy, const __grid_consta
       int ch = tmp % p.chunks_h;
       int b = tmp / p.chunks_h;
       for (int it = 0; it < iters; ++it) {
-        mbar_wait(smem_u32(&bars->empty[st]), ph ^ 1);
+        mbar_wait_quiet(smem_u32(&bars->empty[st]), ph ^ 1);
         const uint32_t full = smem_u32(&bars->full[st]);
         mbar_expect_tx(full, ((p.dbg & 2) ? 0 : ATOM_BYTES) + ((p.dbg & 1) ? 0 : (BN / 128) * ATOM_BYTES));
         const int w0 = cw * p.bw, h0 = ch * p.bh;
@@ -108,10 +108,6 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tm_dy, const __grid_consta
   } else {
     float d[BN / 2];
     const uint32_t a_off = (tid >> 7) * 64 * 128;
-    if (p.dbg & 4) {
-#pragma unroll
-      for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
-    }
     consume_stages<BN>(d, (p.dbg & 4) ? 0 : iters, STAGES, bars->full, bars->empty, p.a_bf16 != 0, 0,
                        [&](uint32_t st, int k, uint64_t& da, uint64_t& db) {
                          const uint32_t a_addr = smem0 + st * STAGE_BYTES;
@@ -119,9 +115,11 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tm_dy, const __grid_consta
                          db = desc_advance_k16(make_desc_k_sw128(a_addr + ATOM_BYTES), k);
                        });
     if (p.dbg & 4) {  // no MMA: the stages still have to be released for the producer
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
       uint32_t st = 0, ph = 0;
       for (int it = 0; it < iters; ++it) {
-        mbar_wait(smem_u32(&bars->full[st]), ph);
+        mbar_wait_quiet(smem_u32(&bars->full[st]), ph);
         __syncwarp();
         if (lane == 0) mbar_arrive(smem_u32(&bars->empty[st]));
         if (++st == STAGES) { st = 0; ph ^= 1; }

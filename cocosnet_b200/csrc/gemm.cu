@@ -67,7 +67,7 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant_
     if (lane == 0) {
       uint32_t st = 0, ph = 0;
       for (int kc = 0; kc < kc_count; ++kc) {
-        mbar_wait(smem_u32(&bars->empty[st]), ph ^ 1);
+        mbar_wait_quiet(smem_u32(&bars->empty[st]), ph ^ 1);
         const uint32_t full = smem_u32(&bars->full[st]);
         mbar_expect_tx(full, STAGE_BYTES);
         tma_load_3d(smem0 + st * STAGE_BYTES, &tm_a, full, kc * BK, m0, bz);

@@ -55,7 +55,9 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     }
   }
 }
-// The same bound without the report: no call inside a wgmma main loop (a call serialises the wgmma pipeline).
+// The same bound without the report, for every wait of a kernel that issues wgmma, its producer warp included: ptxas
+// serialises all wgmma of a kernel that contains a function call (the printf above is one), waiting for each wgmma to
+// complete before the next is issued.
 __device__ __forceinline__ void mbar_wait_quiet(uint32_t bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
@@ -107,26 +109,30 @@ __device__ __forceinline__ void reg_fence(float* d) {
 __device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // Accumulator fragment of m64nN (thread t of the warpgroup: rows 16*(t/32) + (t%32)/4 and +8, column pairs
-// 8j + 2*(t%4)) -> row-major fp32 tile rows [row0, row0 + 64), pitch `ld` floats (even).
+// 8j + 2*(t%4), registers d[4j, 4j + 4)) -> row-major fp32 tile rows [row0, row0 + 64), pitch `ld` floats (even).
+// One 8-column block: fragment block j (d4 = d + 4j) -> tile columns [8 jd, 8 jd + 8).
+__device__ __forceinline__ void acc_block_to_smem(const float* d4, float* tile, int ld, int row0, int jd) {
+  const int t = threadIdx.x & 127;
+  const int r = row0 + 16 * (t >> 5) + ((t & 31) >> 2), c = 8 * jd + 2 * (t & 3);
+  *reinterpret_cast<float2*>(tile + r * ld + c) = make_float2(d4[0], d4[1]);
+  *reinterpret_cast<float2*>(tile + (r + 8) * ld + c) = make_float2(d4[2], d4[3]);
+}
 template <int N>
 __device__ __forceinline__ void acc_to_smem(const float* d, float* tile, int ld, int row0) {
-  const int t = threadIdx.x & 127;
-  const int r = row0 + 16 * (t >> 5) + ((t & 31) >> 2), c = 2 * (t & 3);
 #pragma unroll
-  for (int j = 0; j < N / 8; ++j) {
-    *reinterpret_cast<float2*>(tile + r * ld + 8 * j + c) = make_float2(d[4 * j], d[4 * j + 1]);
-    *reinterpret_cast<float2*>(tile + (r + 8) * ld + 8 * j + c) = make_float2(d[4 * j + 2], d[4 * j + 3]);
-  }
+  for (int j = 0; j < N / 8; ++j) acc_block_to_smem(d + 4 * j, tile, ld, row0, j);
 }
-// 32 consecutive fp32 of a staged accumulator row (16-byte aligned) as raw bits
-__device__ __forceinline__ void acc_ld32(const float* src, uint32_t* r) {
+// N consecutive fp32 of a staged accumulator row (16-byte aligned) as raw bits
+template <int N>
+__device__ __forceinline__ void acc_ld(const float* src, uint32_t* r) {
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
+  for (int i = 0; i < N / 4; ++i) {
     const float4 v = reinterpret_cast<const float4*>(src)[i];
     r[4 * i] = __float_as_uint(v.x); r[4 * i + 1] = __float_as_uint(v.y);
     r[4 * i + 2] = __float_as_uint(v.z); r[4 * i + 3] = __float_as_uint(v.w);
   }
 }
+__device__ __forceinline__ void acc_ld32(const float* src, uint32_t* r) { acc_ld<32>(src, r); }
 
 // --------------------------------------------------------------- descriptors
 // K-major operand tile staged by TMA with SWIZZLE_128B: rows of 64 16-bit elements (128 B), 8-row groups 1024 B apart.
@@ -160,27 +166,56 @@ __device__ __forceinline__ uint64_t desc_advance_k16(uint64_t d, int steps) { re
 constexpr int CONSUMER_WARPS = 8;
 constexpr int TILE_THREADS = 32 * CONSUMER_WARPS + 32;
 
-// d (+)= sum over `iters` stages of 4 K16 steps; desc(st, k, da, db) gives this warpgroup's descriptors.
-template <int BN, typename Desc>
-__device__ __forceinline__ void consume_stages(float* d, int iters, int stages, uint64_t* full, uint64_t* empty,
-                                               bool bf16, int tnsp, Desc desc) {
+// The consumers' position in the ring (stage, phase); a persistent kernel carries it from tile to tile.
+struct RingPos {
   uint32_t st = 0, ph = 0;
+  __device__ __forceinline__ void advance(int stages) {
+    if (++st == static_cast<uint32_t>(stages)) { st = 0; ph ^= 1; }
+  }
+};
+
+// one arrive per consumer warp on `empty`: the stage's buffers go back to the producer
+__device__ __forceinline__ void release_stage(uint64_t* empty) {
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0) mbar_arrive(smem_u32(empty));
+}
+
+// d (+)= sum over `iters` stages of 4 K16 steps; desc(st, k, da, db) gives this warpgroup's descriptors.  One commit
+// group (the 4 wgmmas of a stage) stays in flight while the next stage is waited for and issued: stage s - 1 is
+// released once wait<1> after stage s's commit shows it complete.  The stages are summed in the same order either way.
+template <int BN, bool BF16, typename Desc>
+__device__ __forceinline__ void consume_stages_t(float* d, int iters, int stages, uint64_t* full, uint64_t* empty,
+                                                 int tnsp, Desc desc, RingPos& rp) {
+  uint32_t prev = 0;
   for (int it = 0; it < iters; ++it) {
-    mbar_wait_quiet(smem_u32(&full[st]), ph);
+    mbar_wait_quiet(smem_u32(&full[rp.st]), rp.ph);
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       uint64_t da, db;
-      desc(st, k, da, db);
-      if (bf16) wgmma_ss<BN, true>(d, da, db, (it | k) != 0 ? 1 : 0, tnsp);
-      else wgmma_ss<BN, false>(d, da, db, (it | k) != 0 ? 1 : 0, tnsp);
+      desc(rp.st, k, da, db);
+      wgmma_ss<BN, BF16>(d, da, db, (it | k) != 0 ? 1 : 0, tnsp);
     }
     wgmma_commit();
-    wgmma_wait<0>();
-    __syncwarp();
-    if ((threadIdx.x & 31) == 0) mbar_arrive(smem_u32(&empty[st]));
-    if (++st == static_cast<uint32_t>(stages)) { st = 0; ph ^= 1; }
+    wgmma_wait<1>();
+    if (it > 0) release_stage(&empty[prev]);
+    prev = rp.st;
+    rp.advance(stages);
   }
+  wgmma_wait<0>();
+  if (iters > 0) release_stage(&empty[prev]);
+}
+template <int BN, typename Desc>
+__device__ __forceinline__ void consume_stages(float* d, int iters, int stages, uint64_t* full, uint64_t* empty,
+                                               bool bf16, int tnsp, Desc desc, RingPos& rp) {
+  if (bf16) consume_stages_t<BN, true>(d, iters, stages, full, empty, tnsp, desc, rp);
+  else consume_stages_t<BN, false>(d, iters, stages, full, empty, tnsp, desc, rp);
+}
+template <int BN, typename Desc>
+__device__ __forceinline__ void consume_stages(float* d, int iters, int stages, uint64_t* full, uint64_t* empty,
+                                               bool bf16, int tnsp, Desc desc) {
+  RingPos rp;
+  consume_stages<BN>(d, iters, stages, full, empty, bf16, tnsp, desc, rp);
 }
 
 // After the main loop: both warpgroups write their accumulators into the (drained) operand ring as a row-major fp32

@@ -13,7 +13,8 @@
 //     SBO = 1024 B between 8-pixel groups; a K=16 step advances the start address by 16 pixels = 2048 B.
 //   * X is what the forward saved: fp16.  wgmma cannot mix fp16 x bf16 operands and gradients need the bf16 range,
 //     so the consumer warps convert the landed X atoms fp16 -> bf16 IN PLACE in shared memory (elementwise, so the
-//     swizzle does not matter) and fence to the async proxy before their wgmma reads the stage.
+//     swizzle does not matter) and fence to the async proxy before their wgmma reads the stage.  The main loop keeps
+//     one stage's wgmmas in flight, so stage s + 1 is converted while stage s is multiplied.
 //   * the pixel range is split over the grid (split-K): split k stores its partial tile into slice k of a workspace
 //     and ordered_sum() adds the slices in split order into ws[g][n][c] (same bits on every run; a thread owns 32
 //     consecutive c of one n: 128-byte runs).
@@ -117,7 +118,7 @@ tapwgrad_kernel(const __grid_constant__ CUtensorMap tm_dy, const __grid_constant
       int th_i = tmp % p.tiles_h;
       int b = tmp / p.tiles_h;
       for (int it = 0; it < iters; ++it) {
-        mbar_wait(smem_u32(&bars->empty[st]), ph ^ 1);
+        mbar_wait_quiet(smem_u32(&bars->empty[st]), ph ^ 1);
         const uint32_t full = smem_u32(&bars->full[st]);
         mbar_expect_tx(full, STAGE_BYTES);
         const int w0 = tw_i * p.TW, h0 = th_i * p.TH;
@@ -138,11 +139,14 @@ tapwgrad_kernel(const __grid_constant__ CUtensorMap tm_dy, const __grid_constant
     constexpr int CT = 32 * CONSUMER_WARPS;
     const int wg = tid >> 7;  // output channels [n0 + 64 wg, n0 + 64 wg + 64) = dY atom wg
     float d[BN / 2];
-    uint32_t st = 0, ph = 0;
+    RingPos rp;
+    uint32_t prev = 0;
     for (int it = 0; it < iters; ++it) {
-      mbar_wait_quiet(smem_u32(&bars->full[st]), ph);
+      const uint32_t st = rp.st;
+      mbar_wait_quiet(smem_u32(&bars->full[st]), rp.ph);
       if (p.x_f16) {
-        // ------------------------------------------------------------ converter: X atoms fp16 -> bf16 in place
+        // ------------------------------------------------------------ converter: X atoms fp16 -> bf16 in place,
+        // while the previous stage's wgmmas are still in flight
         uint4* xb = reinterpret_cast<uint4*>(smem_gen + st * STAGE_BYTES + 2 * ATOM);
 #pragma unroll
         for (int i = 0; i < NB * ATOM / 16 / CT; ++i) {
@@ -161,11 +165,13 @@ tapwgrad_kernel(const __grid_constant__ CUtensorMap tm_dy, const __grid_constant
         wgmma_ss<BN, true>(d, da + static_cast<uint64_t>(k * 128), db + static_cast<uint64_t>(k * 128),
                            (it | k) != 0 ? 1 : 0, 1);
       wgmma_commit();
-      wgmma_wait<0>();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&bars->empty[st]));
-      if (++st == STAGES) { st = 0; ph ^= 1; }
+      wgmma_wait<1>();  // one stage in flight; the one before it is complete and goes back to the producer
+      if (it > 0) release_stage(&bars->empty[prev]);
+      prev = st;
+      rp.advance(STAGES);
     }
+    wgmma_wait<0>();
+    release_stage(&bars->empty[prev]);
     const float* tile = stage_acc<BN>(d, smem_gen);
     // ------------------------------------------------------------------ epilogue
     if (warp < 4) {
