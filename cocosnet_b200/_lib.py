@@ -63,6 +63,10 @@ SIGNATURES = {
     "cocos_colsum_nhwc": [_vp, _c_int, _c_int, _c_int, _c_ll, _vp, _vp, _vp, _vp],
     "cocos_gemm_f16": [_vp, _vp, _vp, _c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _c_ll, _c_ll, _c_ll,
                        _c_float, _c_int, _c_int, _vp],
+    "cocos_se_nhwc_fwd": [_vp, _c_int, _c_int, _vp, _c_int, _c_int, _vp, _vp, _vp, _c_int, _c_int, _vp, _vp, _vp]
+                         + [_c_int] * 4 + [_vp, _vp, _vp],
+    "cocos_se_nhwc_bwd": [_vp, _c_int, _vp, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _c_int, _vp, _vp]
+                         + [_c_int] * 4 + [_vp, _vp, _vp],
 }
 
 _lib = None

@@ -348,4 +348,26 @@ int cocos_colsum_nhwc(const void* x, int kind, int Cs, int C, long long rows, fl
   return colsum_nhwc_launch(x, kind, Cs, C, rows, out, ws, ws_floats, static_cast<cudaStream_t>(stream));
 }
 
+int cocos_se_nhwc_fwd(const void* dx, int dx_kind, int dx_Cs, const void* res, int res_kind, int res_Cs, const float* w1,
+                      const float* w2, void* y, int y_kind, int y_Cs, float* m, float* hid, float* s, int B, int C, int Cr,
+                      int HW, float* ws, long long* ws_floats, void* stream) {
+  if (ws && (!dx || !res || !w1 || !w2 || !y || !m || !hid || !s)) {
+    set_error("cocos_se_nhwc_fwd: null pointer argument");
+    return -1;
+  }
+  return se_nhwc_fwd_launch(dx, dx_kind, dx_Cs, res, res_kind, res_Cs, w1, w2, y, y_kind, y_Cs, m, hid, s, B, C, Cr, HW,
+                            ws, ws_floats, static_cast<cudaStream_t>(stream));
+}
+
+int cocos_se_nhwc_bwd(const void* dy, int dy_Cs, const void* dx, int dx_kind, int dx_Cs, const float* w1, const float* w2,
+                      const float* m, const float* hid, const float* s, void* ddx, int ddx_Cs, float* dw1, float* dw2,
+                      int B, int C, int Cr, int HW, float* ws, long long* ws_floats, void* stream) {
+  if (ws && (!dy || !dx || !w1 || !w2 || !m || !hid || !s || !ddx || !dw1 || !dw2)) {
+    set_error("cocos_se_nhwc_bwd: null pointer argument");
+    return -1;
+  }
+  return se_nhwc_bwd_launch(dy, dy_Cs, dx, dx_kind, dx_Cs, w1, w2, m, hid, s, ddx, ddx_Cs, dw1, dw2, B, C, Cr, HW, ws,
+                            ws_floats, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

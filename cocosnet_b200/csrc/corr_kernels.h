@@ -106,4 +106,11 @@ int colsum_nhwc_launch(const void* x, int kind, int Cs, int C, long long rows, f
 int pack_w_launch(const float* w, int Cout, int Cin, int KS, void* dst, int rows, int rows_alloc, int Kc, int ngroups,
                   const signed char* r, const signed char* s, const signed char* term, int transposed, int bf16,
                   cudaStream_t stream);
+int se_nhwc_fwd_launch(const void* dx, int dx_kind, int dx_Cs, const void* res, int res_kind, int res_Cs,
+                       const float* w1, const float* w2, void* y, int y_kind, int y_Cs, float* m, float* hid, float* s,
+                       int B, int C, int Cr, int HW, float* ws, long long* ws_floats, cudaStream_t stream);
+int se_nhwc_bwd_launch(const void* dy, int dy_Cs, const void* dx, int dx_kind, int dx_Cs, const float* w1,
+                       const float* w2, const float* m, const float* hid, const float* s, void* ddx, int ddx_Cs,
+                       float* dw1, float* dw2, int B, int C, int Cr, int HW, float* ws, long long* ws_floats,
+                       cudaStream_t stream);
 }  // namespace cocos

@@ -1,8 +1,9 @@
 // HBM-bound elementwise / normalisation kernels of the 16-bit NHWC pipeline (everything between two tap
 // convolutions), sm_90a.  Tensor "kinds": 1 = fp16, 2 = bf16, 3 = fp32; activations NHWC [B, H, W, Cs] with channel
 // stride Cs >= C; gradients bf16.  `op` tensors (the A operand of the next convolution) are fp16, optionally carry
-// a 1-pixel reflection halo ([B, H+2, W+2, Cs]) and optionally a second fp16 term lo = x - fp16(x) at channel
-// offset lo_off (2-term split operands of the correspondence path).
+// a reflection halo of p pixels ([B, H+2p, W+2p, Cs], p < H, W: F.pad(mode="reflect"); p = dilation of the SPADE block
+// that reads it, 1, 2 or 4) and optionally a second fp16 term lo = x - fp16(x) at channel offset lo_off (2-term split
+// operands of the correspondence path).  Halo gradients are folded back by the exact adjoint of the padding.
 //
 //   spade_mod_nhwc   : PONO + SPADE modulation + LeakyReLU + ReflectionPad2d (normalization.py:63-68,149;
 //                      architecture.py:73-74,94-95) raw -> op, forward / backward
@@ -30,6 +31,7 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+// source index of padded coordinate i + pad, i in [-pad, n + pad), pad < n (one reflection per side)
 __device__ __forceinline__ int reflect1(int i, int n) {
   if (i < 0) i = -i;
   if (i >= n) i = 2 * (n - 1) - i;
@@ -165,7 +167,8 @@ struct SpadeBwd {
   float slope;
 };
 
-// gradient of the padded output folded back onto source pixel (h, w): up to 3 x 3 halo images
+// gradient of the padded output folded back onto source pixel (h, w): up to 3 x 3 halo images (pad < H, W: at most
+// one mirror image per side and dimension)
 struct Fold {
   int hc[3], wc[3], nh, nw;
 };
@@ -948,6 +951,157 @@ __global__ void __launch_bounds__(256) pack_w_kernel(const PackW p) {
   }
 }
 
+// ----------------------------------------------------------------------------------------------- squeeze-excitation
+// SELayer (architecture.py:182-197) on the raw output dx of a SPADE block's conv_1, fused with the block's residual sum:
+// y = res + s[b, c] * dx with s = sigmoid(W2 relu(W1 mean_hw(dx))), W1 [Cr, C], W2 [C, Cr] (bias-free nn.Linear).
+
+// s[b] = sigmoid(W2 relu(W1 m[b])) with m = the per-(image, channel) sums of cocos_in_stats_nhwc / HW: one block per
+// image; m and the hidden activations are kept for the backward.  Every sum runs in a fixed order.
+__global__ void __launch_bounds__(256)
+se_excite_kernel(const float* __restrict__ stats, const float* __restrict__ w1, const float* __restrict__ w2, int C,
+                 int Cr, float inv_hw, float* __restrict__ m, float* __restrict__ hid, float* __restrict__ s) {
+  extern __shared__ float sh[];  // m [C] | hidden [Cr]
+  const int b = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    const float v = stats[(static_cast<size_t>(b) * C + c) * 2] * inv_hw;
+    sh[c] = v;
+    m[static_cast<size_t>(b) * C + c] = v;
+  }
+  __syncthreads();
+  for (int j = warp; j < Cr; j += blockDim.x >> 5) {
+    float t = 0.f;
+    for (int c = lane; c < C; c += 32) t = fmaf(w1[static_cast<size_t>(j) * C + c], sh[c], t);
+    t = fmaxf(warp_sum(t), 0.f);
+    if (lane == 0) {
+      sh[C + j] = t;
+      hid[static_cast<size_t>(b) * Cr + j] = t;
+    }
+  }
+  __syncthreads();
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    float z = 0.f;
+    for (int j = 0; j < Cr; ++j) z = fmaf(w2[static_cast<size_t>(c) * Cr + j], sh[C + j], z);
+    s[static_cast<size_t>(b) * C + c] = 1.f / (1.f + expf(-z));
+  }
+}
+
+// y[b, p, c] = res[b, p, c] + s[b, c] * dx[b, p, c]; one thread per 4 channels of a pixel
+__global__ void __launch_bounds__(256)
+se_apply_nhwc_kernel(const void* __restrict__ dx, int dx_kind, int dx_Cs, const void* __restrict__ res, int res_kind,
+                     int res_Cs, const float* __restrict__ s, void* __restrict__ y, int y_kind, int y_Cs, int C, int HW,
+                     long long n) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int c4 = C >> 2;
+  const long long px = i / c4;
+  const int c = static_cast<int>(i - px * c4) * 4;
+  const float4 v = ld4(dx, dx_kind, px * dx_Cs + c), r = ld4(res, res_kind, px * res_Cs + c);
+  const float4 g = *reinterpret_cast<const float4*>(s + (px / HW) * C + c);
+  st4(y, y_kind, px * y_Cs + c, make_float4(fmaf(g.x, v.x, r.x), fmaf(g.y, v.y, r.y), fmaf(g.z, v.z, r.z),
+                                            fmaf(g.w, v.w, r.w)));
+}
+
+// part[chunk][b][c] = sum over the chunk's pixels of dx * dy (dy bf16): the gradient of the gate; ordered_sum() adds
+// the chunks.  Grid / block as in_stats_nhwc_kernel.
+__global__ void __launch_bounds__(256)
+se_dot_nhwc_kernel(const void* __restrict__ dx, int dx_kind, int dx_Cs, const void* __restrict__ dy, int dy_Cs, int C,
+                   int HW, int pix_per_block, float* __restrict__ part) {
+  __shared__ float red[8][32][4];
+  const int b = blockIdx.z;
+  const int c = (blockIdx.y * blockDim.x + threadIdx.x) * 4;
+  const int p0 = blockIdx.x * pix_per_block;
+  const int p1 = p0 + pix_per_block < HW ? p0 + pix_per_block : HW;
+  float s[4] = {0.f, 0.f, 0.f, 0.f};
+  if (c < C) {
+#pragma unroll 4
+    for (int pix = p0 + threadIdx.y; pix < p1; pix += 8) {
+      const size_t px = static_cast<size_t>(b) * HW + pix;
+      const float4 v = ld4(dx, dx_kind, px * dx_Cs + c), d = ld4(dy, 2, px * dy_Cs + c);
+      s[0] = fmaf(v.x, d.x, s[0]); s[1] = fmaf(v.y, d.y, s[1]); s[2] = fmaf(v.z, d.z, s[2]); s[3] = fmaf(v.w, d.w, s[3]);
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < 4; ++j) red[threadIdx.y][threadIdx.x][j] = s[j];
+  __syncthreads();
+  if (threadIdx.y == 0 && c < C) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      float a = 0.f;
+#pragma unroll
+      for (int k = 0; k < 8; ++k) a += red[k][threadIdx.x][j];
+      if (c + j < C) part[(static_cast<size_t>(blockIdx.x) * gridDim.z + b) * C + c + j] = a;
+    }
+  }
+}
+
+// backward of the gate of image b from ds = sum_hw dx * dy: e2 = ds s (1 - s) (before the sigmoid), e1 = relu'(hid)
+// (W2^T e2) (before the ReLU), dm = W1^T e1 / HW (what every pixel of dx receives through the mean)
+__global__ void __launch_bounds__(256)
+se_excite_bwd_kernel(const float* __restrict__ ds, const float* __restrict__ s, const float* __restrict__ hid,
+                     const float* __restrict__ w1, const float* __restrict__ w2, int C, int Cr, float inv_hw,
+                     float* __restrict__ e2, float* __restrict__ e1, float* __restrict__ dm) {
+  extern __shared__ float sh[];  // e2 [C] | e1 [Cr]
+  const int b = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    const size_t i = static_cast<size_t>(b) * C + c;
+    const float sv = s[i], v = ds[i] * sv * (1.f - sv);
+    sh[c] = v;
+    e2[i] = v;
+  }
+  __syncthreads();
+  for (int j = warp; j < Cr; j += blockDim.x >> 5) {
+    float t = 0.f;
+    for (int c = lane; c < C; c += 32) t = fmaf(w2[static_cast<size_t>(c) * Cr + j], sh[c], t);
+    t = warp_sum(t);
+    if (lane == 0) {
+      const float v = hid[static_cast<size_t>(b) * Cr + j] > 0.f ? t : 0.f;
+      sh[C + j] = v;
+      e1[static_cast<size_t>(b) * Cr + j] = v;
+    }
+  }
+  __syncthreads();
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    float t = 0.f;
+    for (int j = 0; j < Cr; ++j) t = fmaf(w1[static_cast<size_t>(j) * C + c], sh[C + j], t);
+    dm[static_cast<size_t>(b) * C + c] = t * inv_hw;
+  }
+}
+
+// dW1[j, c] = sum_b e1[b, j] m[b, c] and dW2[c, j] = sum_b e2[b, c] hid[b, j], images in ascending order
+__global__ void __launch_bounds__(256)
+se_wgrad_kernel(const float* __restrict__ e1, const float* __restrict__ e2, const float* __restrict__ m,
+                const float* __restrict__ hid, int B, int C, int Cr, float* __restrict__ dw1, float* __restrict__ dw2) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int n = C * Cr;
+  if (i >= 2 * n) return;
+  float t = 0.f;
+  if (i < n) {
+    const int j = i / C, c = i - j * C;
+    for (int b = 0; b < B; ++b) t = fmaf(e1[b * Cr + j], m[static_cast<size_t>(b) * C + c], t);
+    dw1[i] = t;
+  } else {
+    const int k = i - n, c = k / Cr, j = k - c * Cr;
+    for (int b = 0; b < B; ++b) t = fmaf(e2[static_cast<size_t>(b) * C + c], hid[b * Cr + j], t);
+    dw2[k] = t;
+  }
+}
+
+// d dx[b, p, c] = s[b, c] dy[b, p, c] + dm[b, c] (bf16)
+__global__ void __launch_bounds__(256)
+se_dx_nhwc_kernel(const void* __restrict__ dy, int dy_Cs, const float* __restrict__ s, const float* __restrict__ dm,
+                  void* __restrict__ ddx, int ddx_Cs, int C, int HW, long long n) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int c4 = C >> 2;
+  const long long px = i / c4;
+  const int c = static_cast<int>(i - px * c4) * 4;
+  const size_t bc = (px / HW) * C + c;
+  const float4 d = ld4(dy, 2, px * dy_Cs + c);
+  const float4 g = *reinterpret_cast<const float4*>(s + bc), k = *reinterpret_cast<const float4*>(dm + bc);
+  st4(ddx, 2, px * ddx_Cs + c, make_float4(fmaf(g.x, d.x, k.x), fmaf(g.y, d.y, k.y), fmaf(g.z, d.z, k.z),
+                                           fmaf(g.w, d.w, k.w)));
+}
+
 inline int blocks_for(long long n, int per) { return static_cast<int>((n + per - 1) / per); }
 
 }  // namespace
@@ -956,7 +1110,7 @@ inline int blocks_for(long long n, int per) { return static_cast<int>((n + per -
 int spade_mod_nhwc_fwd_launch(const void* x, int x_kind, int x_Cs, const void* gb, int gb_kind, int gb_Cs, void* y,
                               int y_Cs, int y_lo_off, float* mean, float* rstd, int B, int C, int H, int W, int pad,
                               float slope, float eps, cudaStream_t stream) {
-  if (B <= 0 || C < 4 || (C % 4) || H <= pad || W <= pad || pad < 0 || pad > 1 || (x_Cs % 4) || (gb_Cs % 4) ||
+  if (B <= 0 || C < 4 || (C % 4) || H <= pad || W <= pad || pad < 0 || (x_Cs % 4) || (gb_Cs % 4) ||
       (y_Cs % 4) || (y_lo_off % 4) || (x_kind != 1 && x_kind != 3) || (gb_kind != 1 && gb_kind != 3)) {
     set_error("spade_mod_nhwc_fwd: bad arguments (B=%d C=%d H=%d W=%d pad=%d)", B, C, H, W, pad);
     return -1;
@@ -983,7 +1137,7 @@ int spade_mod_nhwc_bwd_launch(const void* dy, int dy_Cs, const void* x, int x_ki
                               int gb_kind, int gb_Cs, int gb_W, const float* mean, const float* rstd, void* dx,
                               int dx_Cs, int dx_acc, void* dgb, int dgb_Cs, int B, int C, int H, int W, int pad,
                               float slope, cudaStream_t stream) {
-  if (B <= 0 || C < 4 || (C % 4) || H <= pad || W <= pad || pad < 0 || pad > 1 || (dy_Cs % 4) || (x_Cs % 4) ||
+  if (B <= 0 || C < 4 || (C % 4) || H <= pad || W <= pad || pad < 0 || (dy_Cs % 4) || (x_Cs % 4) ||
       (gb_Cs % 4) || (dx_Cs % 4) || (dgb_Cs % 4) || (x_kind != 1 && x_kind != 3) || (gb_kind != 1 && gb_kind != 3) ||
       gb_W < 0 || (gb_W && ((gb_W % 4) || (C % gb_W)))) {
     set_error("spade_mod_nhwc_bwd: bad arguments (B=%d C=%d H=%d W=%d pad=%d)", B, C, H, W, pad);
@@ -1034,7 +1188,7 @@ int inst_act_nhwc_fwd_launch(const void* x, int x_kind, int x_Cs, const float* s
                              int y_lo_off, int y_pad, void* y2, int y2_Cs, int B, int C, int H, int W, float eps,
                              const void* gb, int gb_kind, int gb_Cs, int batch_stats, cudaStream_t stream) {
   if (B <= 0 || C <= 0 || (C % 4) || (x_Cs % 4) || (y_Cs % 4) || (y_lo_off % 4) || H <= y_pad || W <= y_pad ||
-      y_pad < 0 || y_pad > 1 || x_kind < 1 || x_kind > 3 || y_kind < 1 || y_kind > 3 || (y_lo_off && y_kind != 1) ||
+      y_pad < 0 || x_kind < 1 || x_kind > 3 || y_kind < 1 || y_kind > 3 || (y_lo_off && y_kind != 1) ||
       (res && (res_kind < 1 || res_kind > 3 || (res_Cs % 4))) || (y2 && (y2_Cs % 4)) ||
       (gb && ((gb_kind != 1 && gb_kind != 3) || (gb_Cs % 4) || gb_Cs < 2 * C))) {
     set_error("inst_act_nhwc_fwd: bad arguments (B=%d C=%d H=%d W=%d pad=%d)", B, C, H, W, y_pad);
@@ -1057,7 +1211,7 @@ int inst_act_nhwc_bwd_launch(const void* dy, int dy_Cs, int dy_pad, const void* 
                              const void* gb, int gb_kind, int gb_Cs, void* dgb, int dgb_Cs, int batch_stats,
                              int const_stats, int phase, float* ws, long long* ws_floats, cudaStream_t stream) {
   if (B <= 0 || C <= 0 || (C % 4) || (dy_Cs % 4) || (x_Cs % 4) || (dx_Cs % 4) || H <= dy_pad || W <= dy_pad ||
-      dy_pad < 0 || dy_pad > 1 || x_kind < 1 || x_kind > 3 || (res && (res_kind < 1 || res_kind > 3 || (res_Cs % 4))) ||
+      dy_pad < 0 || x_kind < 1 || x_kind > 3 || (res && (res_kind < 1 || res_kind > 3 || (res_Cs % 4))) ||
       (dy2 && (dy2_Cs % 4)) || (dres && (dres_Cs % 4)) || !bstats || phase < 0 || phase > 2 ||
       (gb && ((gb_kind != 1 && gb_kind != 3) || (gb_Cs % 4) || gb_Cs < 2 * C || !dgb || (dgb_Cs % 4) || dgb_Cs < 2 * C))) {
     set_error("inst_act_nhwc_bwd: bad arguments (B=%d C=%d H=%d W=%d pad=%d)", B, C, H, W, dy_pad);
@@ -1119,7 +1273,7 @@ int inst_act_nhwc_bwd_launch(const void* dy, int dy_Cs, int dy_pad, const void* 
 int act_bwd_nhwc_launch(const void* dy, int dy_Cs, const void* y, int y_kind, int y_Cs, int pad, void* dz, int dz_Cs,
                         int B, int C, int H, int W, int act, float slope, cudaStream_t stream) {
   if (B <= 0 || C <= 0 || (C % 4) || (dy_Cs % 4) || (y_Cs % 4) || (dz_Cs % 4) || H <= pad || W <= pad || pad < 0 ||
-      pad > 1 || y_kind < 1 || y_kind > 3 || (act != 1 && act != 2)) {
+      y_kind < 1 || y_kind > 3 || (act != 1 && act != 2)) {
     set_error("act_bwd_nhwc: bad arguments (B=%d C=%d H=%d W=%d pad=%d act=%d)", B, C, H, W, pad, act);
     return -1;
   }
@@ -1133,7 +1287,7 @@ int act_bwd_nhwc_launch(const void* dy, int dy_Cs, const void* y, int y_kind, in
 int nhwc_pack_launch(const float* src, void* dst, int kind, int B, int C, int Cs, int lo_off, int c_lo, int c_span,
                      int Hs, int Ws, int H, int W, int f, int pad, cudaStream_t stream) {
   if (B <= 0 || C <= 0 || Cs < C || H <= pad || W <= pad || f < 1 || (H - 1) * f >= Hs || (W - 1) * f >= Ws || pad < 0 ||
-      pad > 1 || kind < 1 || kind > 3 || (lo_off && (kind != 1 || lo_off < C || 2 * lo_off != Cs)) || c_lo < 0 ||
+      kind < 1 || kind > 3 || (lo_off && (kind != 1 || lo_off < C || 2 * lo_off != Cs)) || c_lo < 0 ||
       c_span < 0 || (c_span && (c_span < C || c_lo + c_span > (lo_off ? lo_off : Cs)))) {
     set_error("nhwc_pack: bad arguments (B=%d C=%d Cs=%d c_lo=%d c_span=%d Hs=%d Ws=%d H=%d W=%d f=%d pad=%d)", B, C, Cs,
               c_lo, c_span, Hs, Ws, H, W, f, pad);
@@ -1152,7 +1306,7 @@ int nhwc_pack_launch(const float* src, void* dst, int kind, int B, int C, int Cs
 int nhwc_unpack_launch(const void* src, int kind, int Cs, int c_lo, int C, int B, int H, int W, int pad, float* dst,
                        int Cd, int cd_lo, int Hd, int Wd, int f, int acc, cudaStream_t stream) {
   if (B <= 0 || C <= 0 || c_lo < 0 || c_lo + C > Cs || cd_lo < 0 || cd_lo + C > Cd || H <= pad || W <= pad || f < 1 ||
-      (H - 1) * f >= Hd || (W - 1) * f >= Wd || pad < 0 || pad > 1 || kind < 1 || kind > 3) {
+      (H - 1) * f >= Hd || (W - 1) * f >= Wd || pad < 0 || kind < 1 || kind > 3) {
     set_error("nhwc_unpack: bad arguments (B=%d C=%d Cs=%d H=%d W=%d f=%d pad=%d)", B, C, Cs, H, W, f, pad);
     return -1;
   }
@@ -1290,6 +1444,66 @@ int pack_w_launch(const float* w, int Cout, int Cin, int KS, void* dst, int rows
                                           static_cast<int>(smem)));
   }
   pack_w_kernel<<<dim3((n_in + 31) / 32, (n_out + 31) / 32), dim3(32, 8), smem, stream>>>(p);
+  COCOS_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+static bool se_bad_shape(int B, int C, int Cr, int HW) {
+  return B <= 0 || C < 4 || C > 4096 || (C % 4) || Cr <= 0 || Cr > C || HW <= 0;
+}
+
+int se_nhwc_fwd_launch(const void* dx, int dx_kind, int dx_Cs, const void* res, int res_kind, int res_Cs,
+                       const float* w1, const float* w2, void* y, int y_kind, int y_Cs, float* m, float* hid, float* s,
+                       int B, int C, int Cr, int HW, float* ws, long long* ws_floats, cudaStream_t stream) {
+  if (se_bad_shape(B, C, Cr, HW) || (dx_Cs % 4) || (res_Cs % 4) || (y_Cs % 4) || dx_Cs < C || res_Cs < C || y_Cs < C ||
+      (dx_kind != 1 && dx_kind != 3) || (res_kind != 1 && res_kind != 3) || (y_kind != 1 && y_kind != 3)) {
+    set_error("se_nhwc_fwd: bad arguments (B=%d C=%d Cr=%d HW=%d)", B, C, Cr, HW);
+    return -1;
+  }
+  // workspace: the [B, C, 2] statistics of cocos_in_stats_nhwc, then its own partials
+  const long long nstats = 2ll * B * C;
+  long long need = 0;
+  int rc = in_stats_nhwc_launch(dx, dx_kind, dx_Cs, B, C, HW, nullptr, nullptr, &need, stream);
+  if (rc) return rc;
+  const int wc = workspace_check(ws, ws_floats, nstats + need, "se_nhwc_fwd");
+  if (wc) return wc < 0 ? -1 : 0;
+  if ((rc = in_stats_nhwc_launch(dx, dx_kind, dx_Cs, B, C, HW, ws, ws + nstats, &need, stream))) return rc;
+  se_excite_kernel<<<B, 256, (C + Cr) * sizeof(float), stream>>>(ws, w1, w2, C, Cr, 1.f / HW, m, hid, s);
+  COCOS_CUDA_CHECK(cudaGetLastError());
+  const long long n = static_cast<long long>(B) * HW * (C / 4);
+  se_apply_nhwc_kernel<<<blocks_for(n, 256), 256, 0, stream>>>(dx, dx_kind, dx_Cs, res, res_kind, res_Cs, s, y, y_kind,
+                                                               y_Cs, C, HW, n);
+  COCOS_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+int se_nhwc_bwd_launch(const void* dy, int dy_Cs, const void* dx, int dx_kind, int dx_Cs, const float* w1,
+                       const float* w2, const float* m, const float* hid, const float* s, void* ddx, int ddx_Cs,
+                       float* dw1, float* dw2, int B, int C, int Cr, int HW, float* ws, long long* ws_floats,
+                       cudaStream_t stream) {
+  if (se_bad_shape(B, C, Cr, HW) || (dy_Cs % 4) || (dx_Cs % 4) || (ddx_Cs % 4) || dy_Cs < C || dx_Cs < C ||
+      ddx_Cs < C || (dx_kind != 1 && dx_kind != 3)) {
+    set_error("se_nhwc_bwd: bad arguments (B=%d C=%d Cr=%d HW=%d)", B, C, Cr, HW);
+    return -1;
+  }
+  dim3 grid, block;
+  int ppb;
+  stats_grid(HW, C, B, &grid, &block, &ppb);
+  // workspace: ds [B, C] | e2 [B, C] | dm [B, C] | e1 [B, Cr] | per-chunk partials of ds [chunks][B][C]
+  const long long bc = static_cast<long long>(B) * C, fixed = 3 * bc + static_cast<long long>(B) * Cr;
+  const int wc = workspace_check(ws, ws_floats, fixed + grid.x * bc, "se_nhwc_bwd");
+  if (wc) return wc < 0 ? -1 : 0;
+  float *ds = ws, *e2 = ws + bc, *dm = ws + 2 * bc, *e1 = ws + 3 * bc, *part = ws + fixed;
+  se_dot_nhwc_kernel<<<grid, block, 0, stream>>>(dx, dx_kind, dx_Cs, dy, dy_Cs, C, HW, ppb, part);
+  COCOS_CUDA_CHECK(cudaGetLastError());
+  int rc = ordered_sum(part, grid.x, bc, ds, 0, stream);
+  if (rc) return rc;
+  se_excite_bwd_kernel<<<B, 256, (C + Cr) * sizeof(float), stream>>>(ds, s, hid, w1, w2, C, Cr, 1.f / HW, e2, e1, dm);
+  COCOS_CUDA_CHECK(cudaGetLastError());
+  se_wgrad_kernel<<<blocks_for(2ll * C * Cr, 256), 256, 0, stream>>>(e1, e2, m, hid, B, C, Cr, dw1, dw2);
+  COCOS_CUDA_CHECK(cudaGetLastError());
+  const long long n = static_cast<long long>(B) * HW * (C / 4);
+  se_dx_nhwc_kernel<<<blocks_for(n, 256), 256, 0, stream>>>(dy, dy_Cs, s, dm, ddx, ddx_Cs, C, HW, n);
   COCOS_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

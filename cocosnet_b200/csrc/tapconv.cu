@@ -248,15 +248,17 @@ tapconv_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
     const int n0 = tc.n_i * BN;
     const bool ok = (tb < p.TB) && b < p.B && h < p.H && w < p.W;
     const int yh = h * p.y_sh + p.y_oh, yw = w * p.y_sw + p.y_ow;
-    // store targets: the pixel itself, plus its mirror images in the reflection halo
+    // store targets: the pixel itself, plus its mirror images in the reflection halo of width q < y_H, y_W (at most
+    // one per side: padded row q - yh for 1 <= yh <= q, 2 (y_H - 1) - yh + q for y_H - 1 - q <= yh <= y_H - 2)
     int rt[3], ct[3], nr = 0, nc = 0;
-    rt[nr++] = yh + p.y_pad;
-    ct[nc++] = yw + p.y_pad;
-    if (p.y_reflect && p.y_pad == 1) {
-      if (yh == 1) rt[nr++] = 0;
-      if (yh == p.y_H - 2) rt[nr++] = p.y_H + 1;
-      if (yw == 1) ct[nc++] = 0;
-      if (yw == p.y_W - 2) ct[nc++] = p.y_W + 1;
+    const int q = p.y_pad;
+    rt[nr++] = yh + q;
+    ct[nc++] = yw + q;
+    if (p.y_reflect && q) {
+      if (yh >= 1 && yh <= q) rt[nr++] = q - yh;
+      if (yh <= p.y_H - 2 && yh >= p.y_H - 1 - q) rt[nr++] = 2 * (p.y_H - 1) - yh + q;
+      if (yw >= 1 && yw <= q) ct[nc++] = q - yw;
+      if (yw <= p.y_W - 2 && yw >= p.y_W - 1 - q) ct[nc++] = 2 * (p.y_W - 1) - yw + q;
     }
     const size_t spix = (static_cast<size_t>(b) * p.y_H + yh) * p.y_W + yw;
     float mean = 0.f, rstd = 0.f;
@@ -449,7 +451,8 @@ int tapconv_launch(const cocos_tapconv_desc* d, cudaStream_t stream) {
   const int s = d->a_stride;
   if (d->B <= 0 || d->H <= 0 || d->W <= 0 || d->Hin <= 0 || d->Win <= 0 || d->Ca <= 0 || (d->Ca % 8) || d->Cout <= 0 ||
       (s != 1 && s != 2) || (s == 2 && ((d->Hin | d->Win) & 1)) || d->ngroups <= 0 || d->ngroups > MAXG ||
-      d->kchunks <= 0 || d->y_kind < 0 || d->y_kind > 3 || d->y_pad < 0 || d->y_pad > 1 || d->y_Cs <= 0 ||
+      d->kchunks <= 0 || d->y_kind < 0 || d->y_kind > 3 || d->y_pad < 0 || d->y_Cs <= 0 ||
+      (d->y_reflect && (d->y_pad >= d->y_H || d->y_pad >= d->y_W)) ||
       d->y_sh <= 0 || d->y_sw <= 0 || d->act < 0 || d->act > 3 || (d->res && d->res_kind != 1 && d->res_kind != 3) ||
       (d->res && (d->y_sh != 1 || d->y_sw != 1 || d->y_oh || d->y_ow)) || (d->y_lo_off && d->y_kind != 1) ||
       (d->y_kind == 0 && (d->y_pad || d->y_lo_off))) {

@@ -156,9 +156,17 @@ def spade_supported(norm):
     return (norm.pono or stat) and norm.mlp_gamma.kernel_size == (3, 3)
 
 
+def _wide_halos_and_se():
+    """Dilated blocks (reflection halos of 2 and 4 pixels) and squeeze-excitation need entry points a kernel emulation
+    may lack; the native backend has them."""
+    return getattr(nhwc.backend(), "wide_halos_and_se", False)
+
+
 def block_supported(blk):
     norms = [blk.norm_0, blk.norm_1] + ([blk.norm_s] if blk.learned_shortcut else [])
-    return blk.dilation == 1 and not blk.use_se and all(spade_supported(n) for n in norms)
+    variant = blk.dilation != 1 or blk.use_se
+    return blk.dilation in (1, 2, 4) and (not variant or _wide_halos_and_se()) \
+        and all(spade_supported(n) for n in norms)
 
 
 def register_block(ps, blk):
@@ -169,6 +177,9 @@ def register_block(ps, blk):
     if blk.learned_shortcut:
         ps.conv(blk.conv_s)
         ps.spade(blk.norm_s)
+    if blk.use_se:
+        ps.tensor(("se1", id(blk)), blk.se_layar.fc[0].weight)
+        ps.tensor(("se2", id(blk)), blk.se_layar.fc[2].weight)
 
 
 def spade_norm(tp, ps, norm, x, pyr, mode, slope, pad):
@@ -191,16 +202,23 @@ def spade_norm(tp, ps, norm, x, pyr, mode, slope, pad):
 def spade_block(tp, ps, blk, x, pyr, mode, final_act=ACT_NONE, final_slope=0.0, final_op=False):
     """SPADEResnetBlock.forward (architecture.py:70-95); the residual sum (and, for the generator's last block, the
     LeakyReLU in front of conv_img) ride in conv_1's epilogue.  final_op: the result is the operand of the next
-    convolution (fp16, lo term in split mode) instead of a raw activation."""
+    convolution (fp16, lo term in split mode) instead of a raw activation.  A dilated block (dilation d) pads the
+    operands of conv_0 / conv_1 by ReflectionPad2d(d): the SPADE outputs carry a d-pixel halo.  With squeeze-excitation
+    conv_1 writes the raw dx and the SE op adds the shortcut."""
+    d = blk.dilation
     if blk.learned_shortcut:
         xs = T.conv(tp, spade_norm(tp, ps, blk.norm_s, x, pyr, mode, 1.0, 0), ps.w(blk.conv_s), None, out_kind=mode.raw)
     else:
         xs = x
-    h = T.conv(tp, spade_norm(tp, ps, blk.norm_0, x, pyr, mode, 0.2, 1), ps.w(blk.conv_0), ps.b(blk.conv_0),
-               out_kind=mode.raw)
-    return T.conv(tp, spade_norm(tp, ps, blk.norm_1, h, pyr, mode, 0.2, 1), ps.w(blk.conv_1), ps.b(blk.conv_1),
-                  out_kind=F16 if final_op else mode.raw, split_out=final_op and mode.split, res=xs, act=final_act,
-                  slope=final_slope)
+    h = T.conv(tp, spade_norm(tp, ps, blk.norm_0, x, pyr, mode, 0.2, d), ps.w(blk.conv_0), ps.b(blk.conv_0),
+               out_kind=mode.raw, dilation=d)
+    op = spade_norm(tp, ps, blk.norm_1, h, pyr, mode, 0.2, d)
+    if blk.use_se:
+        assert not final_op and final_act == ACT_NONE
+        dx = T.conv(tp, op, ps.w(blk.conv_1), ps.b(blk.conv_1), out_kind=mode.raw, dilation=d)
+        return T.se(tp, dx, xs, ps.t(("se1", id(blk))), ps.t(("se2", id(blk))), mode.raw)
+    return T.conv(tp, op, ps.w(blk.conv_1), ps.b(blk.conv_1), out_kind=F16 if final_op else mode.raw,
+                  split_out=final_op and mode.split, res=xs, act=final_act, slope=final_slope, dilation=d)
 
 
 # ------------------------------------------------------------------------------------------------ SPADE generator
@@ -272,19 +290,32 @@ def generator_forward(net, seg):
 
 
 # ------------------------------------------------------------------------------------------------ domain adaptor
-def _plain_in_layer(layer):
+def _plain_in_layer(layer, dilation=1):
     return isinstance(layer, nn.Sequential) and len(layer) == 2 and isinstance(layer[0], nn.Conv2d) \
         and isinstance(layer[1], nn.InstanceNorm2d) and not layer[1].affine and not layer[1].track_running_stats \
-        and layer[0].padding_mode == "zeros" and layer[0].dilation == (1, 1) and layer[0].groups == 1
+        and layer[0].padding_mode == "zeros" and layer[0].dilation == (dilation, dilation) and layer[0].groups == 1
+
+
+def _adaptor_blocks(net):
+    """The SPADE blocks in order (generator.py:119-127), and the two degridding layers of --dilation_conv."""
+    opt = net.opt
+    blocks = [net.head_0, net.G_middle_0, net.G_middle_1]
+    degrid = []
+    if opt.adaptor_res_deeper:
+        blocks += [net.deeper0, net.deeper1, net.deeper2]
+        if opt.dilation_conv:
+            degrid = [net.degridding0, net.degridding1]
+    return blocks, degrid
 
 
 def adaptor_supported(net, x):
     opt = net.opt
     layers = [net.layer1, net.layer2, net.layer3, net.layer4, net.layer5]
-    blocks = [net.head_0, net.G_middle_0, net.G_middle_1]
+    blocks, degrid = _adaptor_blocks(net)
     return enabled() and _dev_ok(x) and not x.requires_grad \
         and all(_plain_in_layer(l) for l in layers) and all(block_supported(b) for b in blocks) \
-        and not opt.adaptor_nonlocal and not opt.adaptor_res_deeper and x.shape[2] % 8 == 0 and x.shape[3] % 8 == 0
+        and all(_plain_in_layer(l, d) and l[0].stride == (1, 1) for l, d in zip(degrid, (2, 1))) \
+        and not opt.adaptor_nonlocal and x.shape[2] % 8 == 0 and x.shape[3] % 8 == 0
 
 
 def adaptor_forward(net, x, precise=True):
@@ -292,13 +323,13 @@ def adaptor_forward(net, x, precise=True):
     correspondence.py:245-253).  x fp32 NCHW without gradient (label map or image) -> fp32 NCHW features."""
     mode = T.PRECISE if precise else T.FAST
     layers = [net.layer1, net.layer2, net.layer3, net.layer4, net.layer5]
-    blocks = [net.head_0, net.G_middle_0, net.G_middle_1]
+    blocks, degrid = _adaptor_blocks(net)
     # a one-hot label map is exact in fp16: no lo term for the activations, only for the weights (images, the float
     # pose / edge maps of deepfashion / celebahqedge and noised label maps carry one)
     exact = x.shape[1] > 4 and net.opt.dataset_mode not in ("deepfashion", "celebahqedge") and not net.opt.mask_noise
     xsplit = mode.split and not exact
     ps = ParamSet()
-    for l in layers:
+    for l in layers + degrid:
         ps.conv(l[0])
     for blk in blocks:
         register_block(ps, blk)
@@ -316,8 +347,18 @@ def adaptor_forward(net, x, precise=True):
             else:      # layer5: InstanceNorm only -> raw input of the SPADE blocks
                 h, _ = T.inst_act(tp, r, slope=1.0, eps=l[1].eps, out_kind=mode.raw)
         pyr = Pyramid(tp, 0, src, None, xsplit)
-        for blk in blocks:
-            h = spade_block(tp, ps, blk, h, pyr, mode)
+        for i, blk in enumerate(blocks):
+            h = spade_block(tp, ps, blk, h, pyr, mode, final_op=bool(degrid) and i == len(blocks) - 1)
+        for i, l in enumerate(degrid):
+            # degridding0 (3x3, dilation 2, zero padding 2) + InstanceNorm -> operand of degridding1 (3x3, zero
+            # padding 1) + InstanceNorm -> the features; no activation in between (generator.py:97-98,126)
+            c = l[0]
+            r = T.conv(tp, h, ps.w(c), ps.b(c), padding=c.padding[0], dilation=c.dilation[0], out_kind=mode.raw,
+                       wsplit=mode.split)
+            if i == 0:
+                h, _ = T.inst_act(tp, r, slope=1.0, eps=l[1].eps, out_kind=F16, split_out=mode.split)
+            else:
+                h, _ = T.inst_act(tp, r, slope=1.0, eps=l[1].eps, out_kind=mode.raw)
         return [T.unpack_out(tp, h)]
     return T.run(body, [x], ps.tensors)[0]
 

@@ -55,42 +55,45 @@ class Group:
         self.dh, self.dw, self.coff, self.r, self.s, self.term = dh, dw, coff, r, s, term
 
 
-def plan_fwd(ks, padding, lo_off=0, wsplit=None):
-    """Forward conv (any stride): one group per filter tap; with 2-term split operands up to three
-    (x_hi*W_hi + x_lo*W_hi + x_hi*W_lo).  lo_off: channel offset of x's lo term (0: x is a single fp16 term);
-    wsplit: also use the lo term of the weights (default: whenever x is split)."""
+def plan_fwd(ks, padding, lo_off=0, wsplit=None, dilation=1):
+    """Forward conv (any stride): one group per filter tap at offset r * dilation - padding; with 2-term split operands
+    up to three (x_hi*W_hi + x_lo*W_hi + x_hi*W_lo).  lo_off: channel offset of x's lo term (0: x is a single fp16
+    term); wsplit: also use the lo term of the weights (default: whenever x is split)."""
     wsplit = bool(lo_off) if wsplit is None else wsplit
     groups = []
     for r in range(ks):
         for s in range(ks):
-            groups.append(Group(r - padding, s - padding, 0, r, s, 0))
+            dh, dw = r * dilation - padding, s * dilation - padding
+            groups.append(Group(dh, dw, 0, r, s, 0))
             if lo_off:
-                groups.append(Group(r - padding, s - padding, lo_off, r, s, 0))
+                groups.append(Group(dh, dw, lo_off, r, s, 0))
             if wsplit:
-                groups.append(Group(r - padding, s - padding, 0, r, s, 1))
+                groups.append(Group(dh, dw, 0, r, s, 1))
     return groups
 
 
-def plan_dgrad(ks, padding, stride):
+def plan_dgrad(ks, padding, stride, dilation=1):
     """Backward-data as tap convolutions over dY: list of (pi, pj, groups); stride 1: one class, stride 2: the four
-    input-pixel parity classes.  dX[s*a + pi] = sum_r dY[a + (pi + padding - r)/s] W[r] over the r of matching parity."""
+    input-pixel parity classes.  dX[s*a + pi] = sum_r dY[a + (pi + padding - r*d)/s] W[r] over the r of matching
+    parity (d = dilation)."""
     classes = []
     for pi in range(stride):
         for pj in range(stride):
             groups = []
             for r in range(ks):
-                if (pi + padding - r) % stride:
+                if (pi + padding - r * dilation) % stride:
                     continue
                 for s in range(ks):
-                    if (pj + padding - s) % stride:
+                    if (pj + padding - s * dilation) % stride:
                         continue
-                    groups.append(Group((pi + padding - r) // stride, (pj + padding - s) // stride, 0, r, s, 0))
+                    groups.append(Group((pi + padding - r * dilation) // stride, (pj + padding - s * dilation) // stride,
+                                        0, r, s, 0))
             classes.append((pi, pj, groups))
     return classes
 
 
-def conv_out_size(n_in, ks, padding, stride):
-    return (n_in + 2 * padding - ks) // stride + 1
+def conv_out_size(n_in, ks, padding, stride, dilation=1):
+    return (n_in + 2 * padding - dilation * (ks - 1) - 1) // stride + 1
 
 
 # ------------------------------------------------------------------------------------------------ native backend
@@ -131,6 +134,7 @@ _DTYPES = {F16: torch.float16, BF16: torch.bfloat16, F32: torch.float32}
 class NativeBackend:
     """ctypes -> libcocos_b200.so.  No fallback: constructing it without the library raises."""
     exact = False
+    wide_halos_and_se = True  # reflection halos wider than one pixel (dilated SPADE blocks) and se_fwd / se_bwd
 
     def __init__(self):
         self.lib = _lib.lib()
@@ -302,6 +306,18 @@ class NativeBackend:
                                               dst.data_ptr(), dst.shape[1], cd_lo, dst.shape[2], dst.shape[3], f,
                                               int(acc), _stream()), "cocos_nhwc_unpack")
 
+    def se_fwd(self, dx, res, w1, w2, y, m, hid, s):
+        _lib.call_with_workspace(self.lib.cocos_se_nhwc_fwd, (
+            dx.t.data_ptr(), dx.kind, dx.Cs, res.t.data_ptr(), res.kind, res.Cs, w1.data_ptr(), w2.data_ptr(),
+            y.t.data_ptr(), y.kind, y.Cs, m.data_ptr(), hid.data_ptr(), s.data_ptr(), dx.B, dx.C, w1.shape[0],
+            dx.H * dx.W), _stream(), "cocos_se_nhwc_fwd", kernels=4)
+
+    def se_bwd(self, dy, dx, w1, w2, m, hid, s, ddx, dw1, dw2):
+        _lib.call_with_workspace(self.lib.cocos_se_nhwc_bwd, (
+            dy.t.data_ptr(), dy.Cs, dx.t.data_ptr(), dx.kind, dx.Cs, w1.data_ptr(), w2.data_ptr(), m.data_ptr(),
+            hid.data_ptr(), s.data_ptr(), ddx.t.data_ptr(), ddx.Cs, dw1.data_ptr(), dw2.data_ptr(), dx.B, dx.C,
+            w1.shape[0], dx.H * dx.W), _stream(), "cocos_se_nhwc_bwd", kernels=5)
+
     def colsum(self, x2d, kind, Cs, C, rows, out):
         _lib.call_with_workspace(self.lib.cocos_colsum_nhwc, (x2d.data_ptr(), kind, Cs, C, rows, out.data_ptr()),
                                  _stream(), "cocos_colsum_nhwc", kernels=2)
@@ -462,18 +478,18 @@ def _pack_weight(weight, groups, rows, kc, transposed, bf16, cache=None):
 
 
 def conv(x, weight, bias=None, stride=1, padding=0, act=ACT_NONE, slope=0.0, out_kind=F16, out_pad=0, split_out=False,
-         res=None, nchw_out=None, nchw_coff=0, wsplit=None, scale=None, cache_w=None):
+         res=None, nchw_out=None, nchw_coff=0, wsplit=None, scale=None, cache_w=None, dilation=1):
     """nn.Conv2d forward on the tap-convolution kernel.  x: NT fp16 (its tensor, halo included, IS the conv input;
-    `padding` is the module's zero padding).  scale: 1-element fp32 device tensor multiplied into the accumulator
+    `padding` is the module's zero padding, `dilation` its dilation).  scale: 1-element fp32 device tensor multiplied into the accumulator
     before the bias (spectral norm's 1/sigma: `weight` stays the un-normalised weight_orig).  Returns an NT of kind out_kind (op tensors: out_pad = 1 adds the
-    reflection halo of the next conv, split_out the lo term), or writes fp32 NCHW into `nchw_out` (channels from
+    reflection halo of the next conv, out_pad = d > 1 the halo of a conv with dilation d, split_out the lo term), or writes fp32 NCHW into `nchw_out` (channels from
     nchw_coff) and returns it."""
     assert x.kind == F16, "forward operands are fp16"
     cout, cin, ks, _ = weight.shape
     assert cin == x.C, (cin, x.C)
     hin, win = x.t.shape[1], x.t.shape[2]
-    h, w = conv_out_size(hin, ks, padding, stride), conv_out_size(win, ks, padding, stride)
-    groups = plan_fwd(ks, padding, x.lo, wsplit)
+    h, w = conv_out_size(hin, ks, padding, stride, dilation), conv_out_size(win, ks, padding, stride, dilation)
+    groups = plan_fwd(ks, padding, x.lo, wsplit, dilation)
     kchunks = (cin + 63) // 64
     wp, rows_alloc = _pack_weight(weight, groups, cout, kchunks * 64, False, False, cache=cache_w)
     d = dict(B=x.B, Hin=hin, Win=win, Ca=x.Cs, a_stride=stride, bf16=0, H=h, W=w, Cout=cout, w_rows=rows_alloc,
@@ -508,8 +524,8 @@ def interleave_rows(gamma, beta, W):
 
 
 def conv_spade(actv, weight, bias, x, C, pad, slope, eps=1e-5, split_out=False, want_gb=True, gb_kind=F16, wsplit=None):
-    """SPADE (normalization.py:129-151) + the activation / ReflectionPad2d that follow it (architecture.py:73-74) as
-    ONE convolution launch: `weight` / `bias` are mlp_gamma and mlp_beta interleaved by interleave_rows, actv the
+    """SPADE (normalization.py:129-151) + the activation / ReflectionPad2d(pad) that follow it (architecture.py:73-74;
+    pad = the halo width: the dilation of the convolution that reads y) as ONE convolution launch: `weight` / `bias` are mlp_gamma and mlp_beta interleaved by interleave_rows, actv the
     fp16 operand (relu(mlp_shared(seg)) with its reflection halo), x the raw activation to modulate.  The epilogue
     normalises x per pixel (statistics from one pass of cocos_pono_stats_nhwc), modulates, applies the LeakyReLU and
     writes the operand of the next convolution -- gamma / beta only reach HBM (as `gb`) when the backward needs them.
@@ -538,7 +554,8 @@ def conv_spade(actv, weight, bias, x, C, pad, slope, eps=1e-5, split_out=False, 
     return y, gb, mean, rstd
 
 
-def conv_dgrad(dy, weight, in_hw, stride=1, padding=0, in_pad=0, c_lo=0, c_n=None, scale=None, cache_w=None):
+def conv_dgrad(dy, weight, in_hw, stride=1, padding=0, in_pad=0, c_lo=0, c_n=None, scale=None, cache_w=None,
+               dilation=1):
     """Backward-data: dy NT bf16 [B,H,W,Cout] -> gradient w.r.t. the conv input tensor (halo included) as an NT bf16
     with pad = in_pad (the consumer folds the halo).  in_hw = (Hin, Win) of the input tensor incl. halo.
     c_lo / c_n: only input channels [c_lo, c_lo + c_n) are produced."""
@@ -551,7 +568,7 @@ def conv_dgrad(dy, weight, in_hw, stride=1, padding=0, in_pad=0, c_lo=0, c_n=Non
     wsub = weight if (c_lo == 0 and c_n == cin) else weight[:, c_lo:c_lo + c_n]
     kchunks = (cout + 63) // 64
     out = new(dy.B, hin - 2 * in_pad, win - 2 * in_pad, c_n, BF16, dy.t.device, pad=in_pad)
-    for pi, pj, groups in plan_dgrad(ks, padding, stride):
+    for pi, pj, groups in plan_dgrad(ks, padding, stride, dilation):
         wp, rows_alloc = _pack_weight(wsub, groups, c_n, kchunks * 64, True, True, cache=cache_w if wsub is weight else None)
         hc, wc = (hin - pi + stride - 1) // stride, (win - pj + stride - 1) // stride
         d = dict(B=dy.B, Hin=dy.t.shape[1], Win=dy.t.shape[2], Ca=dy.Cs, a_stride=1, bf16=1, H=hc, W=wc, Cout=c_n,
@@ -566,13 +583,13 @@ def conv_dgrad(dy, weight, in_hw, stride=1, padding=0, in_pad=0, c_lo=0, c_n=Non
 WGRAD_BF16_X = _os.environ.get("COCOS_WGRAD_BF16_X", "1") != "0"
 
 
-def conv_wgrad(dy, x, ks, stride=1, padding=0, scale=None):
+def conv_wgrad(dy, x, ks, stride=1, padding=0, scale=None, dilation=1):
     """Backward-weights: dy NT bf16, x the NT the forward read (fp16, or bf16) -> dW fp32 [Cout, Cin, KS, KS]
     (times the 1-element tensor `scale` when given: it rides in the copy that fixes the layout)."""
     assert dy.kind == BF16 and dy.pad == 0 and x.kind in (F16, BF16)
     if x.kind == F16 and WGRAD_BF16_X:
         x = as_bf16(x)
-    groups = plan_fwd(ks, padding, 0)
+    groups = plan_fwd(ks, padding, 0, dilation=dilation)
     cin, cout = x.C, dy.C
     cin_s = round_up(cin, 4)
     ws = torch.empty((len(groups), cout, cin_s), dtype=torch.float32, device=dy.t.device)
@@ -670,3 +687,28 @@ def inst_act_bwd(dy, x, stats, slope=1.0, slope_ptr=None, res=None, eps=1e-5, dy
         reduce_bstats(bstats)
         backend().inst_bwd(*args, phase=2, **kw)
     return dx, (dres if want_dres else None), dgb
+
+
+# ------------------------------------------------------------------------------------------------ squeeze-excitation
+def se_fwd(dx, res, w1, w2, out_kind):
+    """`x_s + se_layar(dx)` of a SPADE block (architecture.py:88-95,182-197): dx the raw conv_1 output, res the raw
+    shortcut, w1 [C/16, C] / w2 [C, C/16] the bias-free nn.Linear weights (fp32) -> y = res + s * dx (kind out_kind, no
+    halo) with s = sigmoid(W2 relu(W1 mean_hw(dx))).  Returns (y, saved) -- saved = (m, hid, s) for se_bwd."""
+    assert dx.pad == 0 and res.pad == 0 and dx.C == res.C and dx.kind in (F16, F32) and res.kind in (F16, F32)
+    B, C, cr = dx.B, dx.C, w1.shape[0]
+    assert tuple(w1.shape) == (cr, C) and tuple(w2.shape) == (C, cr) and tuple(res.t.shape[:3]) == tuple(dx.t.shape[:3])
+    y = new(B, dx.H, dx.W, C, out_kind, dx.t.device)
+    f32 = dict(dtype=torch.float32, device=dx.t.device)
+    m, hid, s = torch.empty((B, C), **f32), torch.empty((B, cr), **f32), torch.empty((B, C), **f32)
+    backend().se_fwd(dx, res, w1.contiguous(), w2.contiguous(), y, m, hid, s)
+    return y, (m, hid, s)
+
+
+def se_bwd(dy, dx, w1, w2, saved):
+    """dy bf16 (gradient of y; the shortcut's gradient is dy itself) -> (d dx bf16 NT, dW1, dW2 fp32)."""
+    assert dy.kind == BF16 and dy.pad == 0 and dy.C == dx.C
+    m, hid, s = saved
+    ddx = new(dx.B, dx.H, dx.W, dx.C, BF16, dx.t.device)
+    dw1, dw2 = torch.empty_like(w1), torch.empty_like(w2)
+    backend().se_bwd(dy, dx, w1.contiguous(), w2.contiguous(), m, hid, s, ddx, dw1, dw2)
+    return ddx, dw1, dw2

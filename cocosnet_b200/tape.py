@@ -156,14 +156,14 @@ def unpack_out(tp, x):
 
 
 # ------------------------------------------------------------------------------------------------ ops
-def _conv_backward(x, W, b, dz, stride, padding, dx_ch):
+def _conv_backward(x, W, b, dz, stride, padding, dx_ch, dilation=1):
     """Backward-weights / bias / backward-data of a tap convolution from dz (bf16, no halo)."""
     xv, ks = x.v, W.t.shape[2]
     sc = None if W.scale is None else W.scale.t
     if W.need:
         # with an epilogue scale s the layer computed conv(x, s * W): dL/dW = s * G and dL/ds = <G, W>, where
         # G = dz^T x is what the backward-weights GEMM produces (the s * lands in its layout-fixing copy)
-        gw = nhwc.conv_wgrad(dz, xv, ks, stride=stride, padding=padding, scale=sc)
+        gw = nhwc.conv_wgrad(dz, xv, ks, stride=stride, padding=padding, scale=sc, dilation=dilation)
         if W.sn is not None:
             # spectral norm, s = 1 / (u^T W v) with u, v constant: dL/dW = s G - s^2 <G, W> u v^T, and gw = s G
             u, v = W.sn
@@ -177,12 +177,12 @@ def _conv_backward(x, W, b, dz, stride, padding, dx_ch):
     if x.need:
         c_lo, c_n = dx_ch if dx_ch is not None else (0, None)
         dx = nhwc.conv_dgrad(dz, W.t, (xv.t.shape[1], xv.t.shape[2]), stride=stride, padding=padding,
-                             in_pad=xv.pad, c_lo=c_lo, c_n=c_n, scale=sc, cache_w=W.cache)
+                             in_pad=xv.pad, c_lo=c_lo, c_n=c_n, scale=sc, cache_w=W.cache, dilation=dilation)
         acc(x, dx)
 
 
 def conv(tp, x, W, b=None, stride=1, padding=0, act=ACT_NONE, slope=0.0, out_kind=F16, out_pad=0, split_out=False,
-         res=None, dx_ch=None, wsplit=None, nchw=False):
+         res=None, dx_ch=None, wsplit=None, nchw=False, dilation=1):
     """nn.Conv2d on the tap-convolution kernels, forward + (recorded) backward-data / backward-weights.
     res: Var added in the epilogue (before the activation).  dx_ch = (c_lo, n): only those input channels get a
     gradient.  nchw=True: the result is a fp32 NCHW Function output (returned as a torch tensor)."""
@@ -190,23 +190,23 @@ def conv(tp, x, W, b=None, stride=1, padding=0, act=ACT_NONE, slope=0.0, out_kin
     xv = x.v
     sc = None if W.scale is None else W.scale.t
     if nchw:
-        h = nhwc.conv_out_size(xv.t.shape[1], ks, padding, stride)
-        w = nhwc.conv_out_size(xv.t.shape[2], ks, padding, stride)
+        h = nhwc.conv_out_size(xv.t.shape[1], ks, padding, stride, dilation)
+        w = nhwc.conv_out_size(xv.t.shape[2], ks, padding, stride, dilation)
         y = torch.empty((xv.B, W.t.shape[0], h, w), dtype=torch.float32, device=xv.t.device)
         nhwc.conv(xv, W.t, None if b is None else b.t, stride=stride, padding=padding, act=act, slope=slope,
-                  nchw_out=y, wsplit=wsplit, scale=sc, cache_w=W.cache)
+                  nchw_out=y, wsplit=wsplit, scale=sc, cache_w=W.cache, dilation=dilation)
         out = None
     else:
         y = nhwc.conv(xv, W.t, None if b is None else b.t, stride=stride, padding=padding, act=act, slope=slope,
                       out_kind=out_kind, out_pad=out_pad, split_out=split_out, res=None if res is None else res.v,
-                      wsplit=wsplit, scale=sc, cache_w=W.cache)
+                      wsplit=wsplit, scale=sc, cache_w=W.cache, dilation=dilation)
         out = Var(y)
 
     def backward_from(dz):
         """dz: bf16 NT, no halo, gradient of the pre-activation conv output."""
         if res is not None and res.need:
             acc(res, dz)
-        _conv_backward(x, W, b, dz, stride, padding, dx_ch)
+        _conv_backward(x, W, b, dz, stride, padding, dx_ch, dilation)
 
     if nchw:
         def seed(g):
@@ -265,6 +265,28 @@ def spade_conv(tp, x, actv, W, b, C, pad, slope, split, wsplit=None, gb_kind=F16
         if x.need:
             x.g = dx
         _conv_backward(actv, W, b, dgb, 1, 0, None)
+    tp.add(bwd)
+    return out
+
+
+def se(tp, dx, res, w1, w2, out_kind):
+    """SPADEResnetBlock's `x_s + se_layar(dx)` (architecture.py:88-95,182-197): raw dx (conv_1's output), raw res (the
+    shortcut), w1 / w2 the Params of the two bias-free nn.Linear layers -> raw y = res + s * dx (nhwc.se_fwd)."""
+    y, saved = nhwc.se_fwd(dx.v, res.v, w1.t, w2.t, out_kind)
+    out = Var(y)
+
+    def bwd():
+        if out.g is None:
+            return
+        ddx, gw1, gw2 = nhwc.se_bwd(out.g, dx.v, w1.t, w2.t, saved)
+        if dx.need:
+            acc(dx, ddx)
+        if w1.need:
+            w1.add(gw1)
+        if w2.need:
+            w2.add(gw2)
+        if res.need:  # last: acc may hand out.g itself to res
+            acc(res, out.g)
     tp.add(bwd)
     return out
 

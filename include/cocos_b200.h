@@ -23,7 +23,7 @@ extern "C" {
 #define COCOS_ABI_VERSION 7
 
 /* Multi-block reductions (cocos_conv_wgrad, cocos_tapwgrad, cocos_sn_power_iter, cocos_in_stats_nhwc,
- * cocos_inst_act_nhwc_bwd, cocos_pair_loss_nhwc_fwd, cocos_colsum_nhwc) write one partial sum per block into a
+ * cocos_inst_act_nhwc_bwd, cocos_pair_loss_nhwc_fwd, cocos_colsum_nhwc, cocos_se_nhwc_fwd / _bwd) write one partial sum per block into a
  * caller-provided fp32 workspace and add the partials in a fixed order: the same inputs give the same bits on every
  * run.  Workspace arguments (ws, ws_floats): ws == NULL is a size query -- *ws_floats receives the floats needed and
  * nothing is launched; otherwise *ws_floats is the capacity of ws.  The workspace must stay untouched until the work
@@ -170,6 +170,12 @@ int cocos_inst_act_bwd(const float* dy, const float* x, const float* mean, const
  * ------------------------------------------------------------------------------------------------------------------ */
 #define COCOS_TAPCONV_MAX_GROUPS 48
 
+/* Reflection halos: every NHWC entry point below that writes a halo of width pad (y_pad) fills it like
+ * F.pad(mode="reflect"), and every one that reads a haloed gradient folds the halo back by the exact adjoint (each
+ * halo pixel added onto its source).  Any width with pad < H and pad < W is accepted; the networks use 1 and the
+ * dilations 2 and 4 of the dilated SPADE blocks (architecture.py:22-24 with --dilation_conv).
+ * A dilated 3x3 convolution is the same nine tap groups at offsets dh = r*dilation - padding: no separate kernel. */
+
 /* cocos_tapconv: y[b, h, w, n] = epilogue( sum_g sum_{c < 64*kchunks}
  *                    x[b, a_stride*h + dh[g], a_stride*w + dw[g], coff[g] + c] * w[n, (g*kchunks)*64 + c] )
  * Replaces nn.Conv2d forward (architecture.py:31-33,73-74; normalization.py:112-120; correspondence.py:17-22,79-146;
@@ -183,8 +189,9 @@ int cocos_inst_act_bwd(const float* dy, const float* x, const float* mean, const
  *             + res[b,h,w,n] (kind 1 or 3, channel stride res_Cs, may be NULL),
  *             act 0 none / 1 ReLU / 2 LeakyReLU(slope) / 3 tanh.
  *   y   : kind y_kind.  NHWC kinds: [B, y_H + 2*y_pad, y_W + 2*y_pad, y_Cs], channel offset y_coff; output pixel
- *         (h, w) lands at (h*y_sh + y_oh, w*y_sw + y_ow) (+ y_pad); y_reflect fills the 1-pixel halo by reflection
- *         (nn.ReflectionPad2d(1) of the consumer); y_lo_off != 0 (fp16 only) also stores lo = v - fp16(v) at channel
+ *         (h, w) lands at (h*y_sh + y_oh, w*y_sw + y_ow) (+ y_pad); y_reflect fills the y_pad-pixel halo by
+ *         reflection (nn.ReflectionPad2d(y_pad) of the consumer: 1, or the dilation 2 / 4 of a dilated SPADE block;
+ *         y_pad < y_H, y_W); y_lo_off != 0 (fp16 only) also stores lo = v - fp16(v) at channel
  *         offset + y_lo_off (2-term split operand).  y_kind 0: fp32 NCHW [B, y_Cs, y_H, y_W]. */
 typedef struct cocos_tapconv_desc {
   const void* x;
@@ -351,6 +358,21 @@ int cocos_nhwc_unpack(const void* src, int kind, int Cs, int c_lo, int C, int B,
 /* out[c] = sum over the rows of x [rows, Cs] (kind 1|2|3), c < C: the bias gradient of a convolution. */
 int cocos_colsum_nhwc(const void* x, int kind, int Cs, int C, long long rows, float* out, float* ws,
                       long long* ws_floats, void* stream);
+/* Squeeze-excitation (SELayer, architecture.py:182-197) of a SPADE block's raw conv_1 output dx, fused with the
+ * block's residual sum:  y = res + s[b,c] * dx,  s = sigmoid(W2 relu(W1 m)),  m[b,c] = mean over the HW pixels of dx.
+ *   dx (kind 1|3, [B,HW,dx_Cs]), res (kind 1|3), y (kind 1|3, no halo); w1 fp32 [Cr, C], w2 fp32 [C, Cr] (bias-free
+ *   nn.Linear weights, Cr = C / 16); m, s fp32 [B, C] and hid = relu(W1 m) fp32 [B, Cr] are written for the backward.
+ *   The squeeze is cocos_in_stats_nhwc's fixed-order reduction.  C % 4 == 0, C <= 4096.
+ * Backward from dy (bf16, gradient of y; the residual's gradient is dy itself):
+ *   ds[b,c] = sum_hw dy * dx (fixed order), ddx = s * dy + dm[b,c] / HW (bf16, overwritten) with dm the gradient of
+ *   m, dw1 fp32 [Cr, C] and dw2 fp32 [C, Cr] overwritten (images added in ascending order).
+ * Both take the workspace protocol of the multi-block reductions (ws NULL: size query). */
+int cocos_se_nhwc_fwd(const void* dx, int dx_kind, int dx_Cs, const void* res, int res_kind, int res_Cs, const float* w1,
+                      const float* w2, void* y, int y_kind, int y_Cs, float* m, float* hid, float* s, int B, int C, int Cr,
+                      int HW, float* ws, long long* ws_floats, void* stream);
+int cocos_se_nhwc_bwd(const void* dy, int dy_Cs, const void* dx, int dx_kind, int dx_Cs, const float* w1, const float* w2,
+                      const float* m, const float* hid, const float* s, void* ddx, int ddx_Cs, float* dw1, float* dw2,
+                      int B, int C, int Cr, int HW, float* ws, long long* ws_floats, void* stream);
 
 #ifdef __cplusplus
 }
