@@ -308,14 +308,28 @@ def _adaptor_blocks(net):
     return blocks, degrid
 
 
+def attention_supported(attn):
+    """The SAGAN block on the tape (T.attention): four plain bias-free 1x1 convolutions without forward pre-hooks (no
+    spectral norm), at most 256 value channels (K1's limit), and a backend with the non-local entry points."""
+    convs = (attn.theta, attn.phi, attn.g, attn.o)
+    plain = all(isinstance(c, nn.Conv2d) and c.kernel_size == (1, 1) and c.stride == (1, 1) and c.padding == (0, 0)
+                and c.dilation == (1, 1) and c.groups == 1 and c.bias is None and c.padding_mode == "zeros"
+                and not c._forward_pre_hooks for c in convs)
+    return plain and attn.theta.out_channels == attn.phi.out_channels and attn.g.out_channels <= 256 \
+        and getattr(nhwc.backend(), "nonlocal_attention", False)
+
+
 def adaptor_supported(net, x):
     opt = net.opt
     layers = [net.layer1, net.layer2, net.layer3, net.layer4, net.layer5]
     blocks, degrid = _adaptor_blocks(net)
+    # --adaptor_nonlocal: the 2x2 max pooling of the features (x / 4 or x / 2) needs even sizes
+    nonlocal_ok = not opt.adaptor_nonlocal or (attention_supported(net.attn) and x.shape[2] % 16 == 0
+                                               and x.shape[3] % 16 == 0)
     return enabled() and _dev_ok(x) and not x.requires_grad \
         and all(_plain_in_layer(l) for l in layers) and all(block_supported(b) for b in blocks) \
         and all(_plain_in_layer(l, d) and l[0].stride == (1, 1) for l, d in zip(degrid, (2, 1))) \
-        and not opt.adaptor_nonlocal and x.shape[2] % 8 == 0 and x.shape[3] % 8 == 0
+        and nonlocal_ok and x.shape[2] % 8 == 0 and x.shape[3] % 8 == 0
 
 
 def adaptor_forward(net, x, precise=True):
@@ -333,6 +347,11 @@ def adaptor_forward(net, x, precise=True):
         ps.conv(l[0])
     for blk in blocks:
         register_block(ps, blk)
+    attn = net.attn if net.opt.adaptor_nonlocal else None
+    if attn is not None:  # theta | phi | g as one convolution: autograd splits the concatenation's gradient
+        ps.tensor(("attn_tpg", id(attn)), torch.cat((attn.theta.weight, attn.phi.weight, attn.g.weight), 0))
+        ps.conv(attn.o)
+        ps.tensor(("attn_gamma", id(attn)), attn.gamma)
 
     def body(tp, ins, params):
         ps.bind(params)
@@ -349,6 +368,8 @@ def adaptor_forward(net, x, precise=True):
         pyr = Pyramid(tp, 0, src, None, xsplit)
         for i, blk in enumerate(blocks):
             h = spade_block(tp, ps, blk, h, pyr, mode, final_op=bool(degrid) and i == len(blocks) - 1)
+            if attn is not None and blk is net.head_0:  # the SAGAN block after head_0 (generator.py:124-125,148-149)
+                h = T.attention(tp, h, ps.t(("attn_tpg", id(attn))), ps.w(attn.o), ps.t(("attn_gamma", id(attn))), mode)
         for i, l in enumerate(degrid):
             # degridding0 (3x3, dilation 2, zero padding 2) + InstanceNorm -> operand of degridding1 (3x3, zero
             # padding 1) + InstanceNorm -> the features; no activation in between (generator.py:97-98,126)

@@ -135,6 +135,7 @@ class NativeBackend:
     """ctypes -> libcocos_b200.so.  No fallback: constructing it without the library raises."""
     exact = False
     wide_halos_and_se = True  # reflection halos wider than one pixel (dilated SPADE blocks) and se_fwd / se_bwd
+    nonlocal_attention = True  # to_op, attn_pack / attn_do_rows / attn_grad_unpack and K1 / stage A / GEMM behind them
 
     def __init__(self):
         self.lib = _lib.lib()
@@ -321,6 +322,41 @@ class NativeBackend:
     def colsum(self, x2d, kind, Cs, C, rows, out):
         _lib.call_with_workspace(self.lib.cocos_colsum_nhwc, (x2d.data_ptr(), kind, Cs, C, rows, out.data_ptr()),
                                  _stream(), "cocos_colsum_nhwc", kernels=2)
+
+    # ---------------------------------------------------------------------------------------- non-local block
+    def to_op(self, x, y):
+        _lib.check(self.lib.cocos_nhwc_to_op(x.t.data_ptr(), x.kind, x.Cs, y.t.data_ptr(), y.Cs, y.lo,
+                                             x.t.numel() // x.Cs, _stream()), "cocos_nhwc_to_op")
+
+    def attn_pack(self, z, kd, cv, split, q, k, vt, v16, q_cm, k_cm):
+        _lib.check(self.lib.cocos_attn_pack_nhwc(
+            z.t.data_ptr(), z.kind, z.Cs, z.B, z.H, z.W, kd, cv, int(split), q.data_ptr(), k.data_ptr(), vt.data_ptr(),
+            vt.shape[1], vt.stride(1), _p(v16), v16.shape[3] if v16 is not None else 0, _p(q_cm),
+            q_cm.stride(1) if q_cm is not None else round_up(z.H * z.W, 8), _p(k_cm), _stream()),
+            "cocos_attn_pack_nhwc", kernels=2)
+
+    def attend_fwd(self, q, k, vt, cv, nk):
+        from . import ops
+        out, lse, _ = ops.corr_warp_fwd(q, k, vt, cv, nk, 1.0, want_lse=True)
+        return out, lse
+
+    def attend_bwd_ds(self, q, k, do16, rscale, v16, out, lse, cv, want_pt=True):
+        from . import ops
+        return ops.corr_warp_bwd_ds(q, k, do16, rscale, v16, out, lse, cv, 1.0, want_pt)
+
+    def gemm(self, a, b, out=None):
+        from . import ops
+        return ops.gemm_f16(a, b, out=out, accumulate=out is not None)
+
+    def attn_do_rows(self, dy, cv, do16, rscale, do_cm, out, out_ck):
+        _lib.check(self.lib.cocos_attn_do_rows(dy.t.data_ptr(), dy.Cs, dy.B, dy.H * dy.W, cv, do16.data_ptr(),
+                                               do16.shape[3], rscale.data_ptr(), do_cm.data_ptr(), do_cm.stride(1),
+                                               out.data_ptr(), _p(out_ck), _stream()), "cocos_attn_do_rows")
+
+    def attn_grad_unpack(self, dq, dk, dv, z, kd, cv, dz):
+        _lib.check(self.lib.cocos_attn_grad_unpack(dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), z.t.data_ptr(), z.kind,
+                                                   z.Cs, z.B, z.H, z.W, kd, cv, dz.t.data_ptr(), dz.Cs, _stream()),
+                   "cocos_attn_grad_unpack")
 
 
 _BACKEND = None
@@ -712,3 +748,75 @@ def se_bwd(dy, dx, w1, w2, saved):
     dw1, dw2 = torch.empty_like(w1), torch.empty_like(w2)
     backend().se_bwd(dy, dx, w1.contiguous(), w2.contiguous(), m, hid, s, ddx, dw1, dw2)
     return ddx, dw1, dw2
+
+
+# ------------------------------------------------------------------------------------------------ non-local block
+def to_op(x, split=False):
+    """Raw NT (fp32 / fp16, no halo) -> fp16 conv operand of the same geometry (+ the lo term): the SAGAN block's input
+    is both the theta | phi | g operand and the residual (architecture.py:116-118,127)."""
+    assert x.pad == 0 and x.lo == 0 and x.kind in (F16, F32) and x.Cs == round_up(x.C, 8)
+    y = new(x.B, x.H, x.W, x.C, F16, x.t.device, split=split, zero=False)
+    backend().to_op(x, y)
+    return y
+
+
+def attn_chunk(cv):
+    """Value channels per stage-A call of the attend backward: its shared-memory plan takes at most 192 (so 256 value
+    channels -- the adaptor's block, ch = 512 -- run as two calls of 128 whose dS / dS^T the GEMMs add up)."""
+    return round_up(cv, 64) if cv <= 192 else 128
+
+
+def attn_pack(z, kd, cv, split=False, for_backward=True):
+    """Raw output z of the theta | phi | g 1x1 convolution (channels [0, kd) theta, [kd, 2kd) phi, [2kd, 2kd + cv) g)
+    -> (q, k, vt, saved): K1's operands -- theta rows, maxpool2(phi) rows (3-term split layouts when `split`) and
+    maxpool2(g) channel-major -- and, for_backward, saved = (v16, q_cm, k_cm): maxpool2(g) position-major and bf16
+    channel-major theta / maxpool2(phi), the other operands of stage A and the dQ / dK GEMMs (architecture.py:116-122)."""
+    assert z.pad == 0 and z.C == 2 * kd + cv and z.H % 2 == 0 and z.W % 2 == 0
+    be, dev = backend(), z.t.device
+    nq = z.H * z.W
+    nk = nq // 4
+    kt = round_up(kd, 64) * (3 if split else 1)
+    q = be.empty((z.B, nq, kt), F16, dev)
+    k = be.empty((z.B, nk, kt), F16, dev)
+    vt = be.empty((z.B, round_up(cv, 16), round_up(nk, 8)), F16, dev)
+    v16 = q_cm = k_cm = None
+    if for_backward:
+        cvk = attn_chunk(cv)
+        v16 = be.empty(((cv + cvk - 1) // cvk, z.B, nk, cvk), F16, dev)
+        q_cm = be.empty((z.B, kd, round_up(nq, 8)), BF16, dev)[:, :, :nq]
+        k_cm = be.empty((z.B, kd, round_up(nk, 8)), BF16, dev)[:, :, :nk]
+    be.attn_pack(z, kd, cv, split, q, k, vt, v16, q_cm, k_cm)
+    return q, k, vt, (v16, q_cm, k_cm)
+
+
+def attend(q, k, vt, cv):
+    """K1 at scale 1: (out fp32 [B, cv, Nq] = bmm(g, softmax(theta^T phi)^T), lse [B, Nq])."""
+    return backend().attend_fwd(q, k, vt, cv, k.shape[1])
+
+
+def attend_backward(dy, z, kd, cv, q, k, out, lse, saved):
+    """dy: bf16 NT gradient of the attention output ([B, H, W, cv], no halo) -> bf16 NT gradient of z.  Stage A
+    recomputes P from the forward's (split) operands and lse; dQ^T = K_cm dS, dK^T = Q_cm dS^T, dV^T = dO_cm P^T are
+    three bf16 GEMMs; the unpack routes dK / dV through the 2x2 max pooling."""
+    assert dy.kind == BF16 and dy.pad == 0 and dy.C == cv
+    be, dev = backend(), dy.t.device
+    v16, q_cm, k_cm = saved
+    nq = dy.H * dy.W
+    cvk = v16.shape[3]
+    nchunk = v16.shape[0]
+    do16 = be.empty((nchunk, dy.B, nq, cvk), F16, dev)
+    rscale = torch.empty((dy.B, nq), dtype=torch.float32, device=dev)
+    do_cm = be.empty((dy.B, cv, round_up(nq, 8)), BF16, dev)[:, :, :nq]
+    out_ck = torch.empty((nchunk * dy.B * cvk * nq,), dtype=torch.float32, device=dev) if nchunk > 1 else None
+    be.attn_do_rows(dy, cv, do16, rscale, do_cm, out, out_ck)
+    dq = dk = dv = None
+    for c in range(nchunk):  # dS is linear in the value channels: the chunks' dS / dS^T add up in the GEMMs
+        cvc = min(cvk, cv - c * cvk)
+        oc = out if nchunk == 1 else out_ck[c * dy.B * cvk * nq:][:dy.B * cvc * nq].view(dy.B, cvc, nq)
+        ds, dst, pt = be.attend_bwd_ds(q, k, do16[c], rscale, v16[c], oc, lse, cvc, want_pt=c == 0)
+        dq, dk = be.gemm(k_cm, ds, out=dq), be.gemm(q_cm, dst, out=dk)
+        if c == 0:
+            dv = be.gemm(do_cm, pt)
+    dz = new(z.B, z.H, z.W, z.C, BF16, dev, zero=False)
+    be.attn_grad_unpack(dq, dk, dv, z, kd, cv, dz)
+    return dz

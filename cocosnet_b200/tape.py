@@ -160,7 +160,14 @@ def _conv_backward(x, W, b, dz, stride, padding, dx_ch, dilation=1):
     """Backward-weights / bias / backward-data of a tap convolution from dz (bf16, no halo)."""
     xv, ks = x.v, W.t.shape[2]
     sc = None if W.scale is None else W.scale.t
-    if W.need:
+    if sc is not None and W.sn is None and W.scale.need:
+        # a trainable epilogue scale (the SAGAN block's gamma, architecture.py:112,127): dL/ds = <G, W> and
+        # dL/dW = s G from the UNSCALED G -- gamma starts at exactly 0, where <s G, W> / s would be 0 / 0
+        gw = nhwc.conv_wgrad(dz, xv, ks, stride=stride, padding=padding, dilation=dilation)
+        W.scale.add(torch.dot(gw.reshape(-1), W.t.reshape(-1)).reshape(sc.shape))
+        if W.need:
+            W.add(gw.mul_(sc.reshape(())))
+    elif W.need:
         # with an epilogue scale s the layer computed conv(x, s * W): dL/dW = s * G and dL/ds = <G, W>, where
         # G = dz^T x is what the backward-weights GEMM produces (the s * lands in its layout-fixing copy)
         gw = nhwc.conv_wgrad(dz, xv, ks, stride=stride, padding=padding, scale=sc, dilation=dilation)
@@ -169,8 +176,6 @@ def _conv_backward(x, W, b, dz, stride, padding, dx_ch, dilation=1):
             u, v = W.sn
             k = torch.dot(gw.reshape(-1), W.t.reshape(-1)) * sc.reshape(())
             gw.view(gw.shape[0], -1).addcmul_(u[:, None] * (-k), v[None, :])
-        elif sc is not None and W.scale.need:
-            W.scale.add((torch.dot(gw.reshape(-1), W.t.reshape(-1)) / sc.reshape(())).reshape(sc.shape))
         W.add(gw)
     if b is not None and b.need:
         b.add(nhwc.bias_grad(dz))
@@ -289,6 +294,37 @@ def se(tp, dx, res, w1, w2, out_kind):
             acc(res, out.g)
     tp.add(bwd)
     return out
+
+
+def attention(tp, x, w_tpg, w_o, gamma, mode):
+    """The SAGAN non-local block (architecture.py:97-127) without spectral norm:
+    y = x + gamma * o(bmm(g, softmax(theta^T phi)^T)), phi and g max-pooled 2x2, all four convolutions 1x1 and bias-free.
+    x: raw Var (no halo); w_tpg: Param of torch.cat((theta, phi, g) weights) -- ONE tap convolution; w_o, gamma: Params
+    of o's weight and of the gain, which rides in o's epilogue as its scale, with x as the residual.  PRECISE mode: fp32
+    activations and 3-term split Q / K (what corr._Attend(precision="split") does); FAST: single fp16 terms."""
+    xv = x.v
+    cv = w_o.t.shape[1]
+    kd = (w_tpg.t.shape[0] - cv) // 2
+    assert w_tpg.t.shape[2:] == (1, 1) and w_o.t.shape[2:] == (1, 1) and w_o.t.shape[0] == xv.C and xv.pad == 0
+    xop = Var(nhwc.to_op(xv, split=mode.split), need=x.need)
+
+    def cast_bwd():
+        if xop.g is not None and x.need:
+            acc(x, xop.g)
+    tp.add(cast_bwd)
+    z = conv(tp, xop, w_tpg, None, out_kind=mode.raw, wsplit=mode.split)
+    zv = z.v
+    q, k, vt, saved = nhwc.attn_pack(zv, kd, cv, split=mode.split, for_backward=tp.record)
+    out, lse = nhwc.attend(q, k, vt, cv)
+    a = Var(nhwc.pack(out.view(xv.B, cv, xv.H, xv.W), F16, split=mode.split))
+
+    def attend_bwd():
+        if a.g is None:
+            return
+        acc(z, nhwc.attend_backward(a.g, zv, kd, cv, q, k, out, lse, saved))
+    tp.add(attend_bwd)
+    w_o.scale = gamma
+    return conv(tp, a, w_o, None, out_kind=mode.raw, res=x, wsplit=mode.split)
 
 
 def inst_act(tp, x, slope=1.0, prelu=None, res=None, eps=1e-5, out_kind=F16, out_pad=0, split_out=False,

@@ -374,6 +374,48 @@ int cocos_se_nhwc_bwd(const void* dy, int dy_Cs, const void* dx, int dx_kind, in
                       const float* m, const float* hid, const float* s, void* ddx, int ddx_Cs, float* dw1, float* dw2,
                       int B, int C, int Cr, int HW, float* ws, long long* ws_floats, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * SAGAN non-local block (Attention, architecture.py:97-127; the adaptor's --adaptor_nonlocal, generator.py:124-125,
+ * 148-149) on the NHWC tape:  y = x + gamma * o(bmm(g, softmax(theta^T phi)^T)),  phi and g max-pooled 2x2.  The 1x1
+ * convolutions theta | phi | g run as ONE cocos_tapconv with the three filters concatenated (raw output z, channels
+ * [0, Kd) theta, [Kd, 2Kd) phi, [2Kd, 2Kd + Cv) g); the attend step is K1 at scale 1 and its backward stage A plus three
+ * bf16 GEMMs; o runs as a cocos_tapconv with scale = gamma and res = x.  The entry points below are the layout and
+ * gradient steps in between.  None of them reduces across threads: no atomics, no workspace, the same bits every run.
+ * ------------------------------------------------------------------------------------------------------------------ */
+/* Raw NHWC activation x (kind 1|3, [npix, Cs], Cs % 8 == 0, no halo) -> fp16 conv operand y [npix, y_Cs]: hi =
+ * fp16(x) at channels [0, Cs) and, for lo_off != 0, lo = fp16(x - hi) at [lo_off, lo_off + Cs) (2-term split).  The
+ * block's input x is both the theta | phi | g operand and the fp32 residual (architecture.py:116-118,127). */
+int cocos_nhwc_to_op(const void* x, int x_kind, int Cs, void* y, int y_Cs, int lo_off, long long npix, void* stream);
+/* Forward pack of the raw theta | phi | g output z (kind 1|3, [B, H, W, z_Cs], H and W even; Nq = H*W, Nk = Nq/4).
+ * Replaces the view / max_pool2d / transpose steps of architecture.py:116-122 in front of K1.  Kp = Kd rounded up
+ * to 64, Kt = Kp * (split ? 3 : 1):
+ *   q    fp16 [B, Nq, Kt]  theta rows: [hi] or the query layout [hi, lo, hi] (cocos_pack_rows_f16 split mode 1)
+ *   k    fp16 [B, Nk, Kt]  maxpool2(phi) rows: [hi] or the key layout [hi, hi, lo]
+ *   vt   fp16 [B, Cvp, Nkp] maxpool2(g) channel-major, K1's V (Cvp % 16 == 0, Nkp % 8 == 0, zero padded)
+ * and for the backward (all optional; q_cm and k_cm both or neither):
+ *   v16  fp16 [ceil(Cv / Cvk), B, Nk, Cvk] maxpool2(g) position-major in chunks of Cvk channels (Cvk % 64 == 0, zero
+ *        beyond Cv): stage A's V, one cocos_corr_warp_bwd_ds call per chunk (its shared-memory plan takes Cvk <= 192)
+ *   q_cm bf16 [B, Kd, Nqp], k_cm bf16 [B, Kd, Nkp]: theta and maxpool2(phi) channel-major, the A operands of the
+ *        dQ / dK GEMMs (pitches multiples of 8; the padding columns are not written). */
+int cocos_attn_pack_nhwc(const void* z, int z_kind, int z_Cs, int B, int H, int W, int Kd, int Cv, int split, void* q,
+                         void* k, void* vt, int Cvp, int Nkp, void* v16, int Cvk, void* q_cm, int Nqp, void* k_cm,
+                         void* stream);
+/* dO rows of the attend backward from dy, the bf16 NHWC gradient of the attention output ([B, N, dy_Cs], Cv channels;
+ * the gradient of bmm(g, beta^T) in architecture.py:126): do16 fp16 [ceil(Cv / Cvk), B, N, Cvk] = r * dy in chunks of
+ * Cvk channels (Cvk % 64 == 0, zero beyond Cv) with r = 1 / max_c |dy| over all Cv channels (1 for an all-zero row)
+ * written to rscale [B, N] -- what cocos_pack_rows_f16 with rowscale_out makes from fp32 channel-major -- and do_cm
+ * bf16 [B, Cv, Nqp] = dy channel-major, the A operand of the dV GEMM.  With more than one chunk, out_chunks receives
+ * K1's output out fp32 [B, Cv, N] regrouped per chunk (chunk c: [B, cv_c, N] at offset c * B * Cvk * N), the `out`
+ * of each stage-A call; otherwise out / out_chunks may be NULL. */
+int cocos_attn_do_rows(const void* dy, int dy_Cs, int B, int N, int Cv, void* do16, int Cvk, float* rscale, void* do_cm,
+                       int Nqp, const float* out, float* out_chunks, void* stream);
+/* Gradient of the theta | phi | g output from the three GEMM results dq fp32 [B, Kd, Nq], dk fp32 [B, Kd, Nk], dv fp32
+ * [B, Cv, Nk] (channel-major, dense): dz bf16 [B, H, W, dz_Cs] (fully overwritten, zero beyond 2Kd + Cv) with theta's
+ * channels = dq transposed and phi's / g's = dk / dv at the first maximum in scan order of each 2x2 window of z, zero
+ * elsewhere -- the backward of F.max_pool2d (architecture.py:117-118), the argmax recomputed from the saved z. */
+int cocos_attn_grad_unpack(const float* dq, const float* dk, const float* dv, const void* z, int z_kind, int z_Cs, int B,
+                           int H, int W, int Kd, int Cv, void* dz, int dz_Cs, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,0 +1,182 @@
+"""CPU: the SAGAN non-local block of the domain adaptor (--adaptor_nonlocal) on the NHWC tape -- tape.attention through
+the kernel emulation (tests/emul_attn.py) against the mirror module blocks.Attention in fp64 autograd, at gamma != 0
+and at the initial gamma = 0, the 2x2 argmax routing on ties, and the whole 64x64 training step of both
+--adaptor_nonlocal flag sets against goldens minted from the unmodified reference."""
+import os
+
+import numpy as np
+import pytest
+import torch
+
+from cocosnet_b200 import nhwc
+from cocosnet_b200 import tape as T
+from tests.emul_attn import AttnEmulBackend
+
+GOLD = os.path.join(os.path.dirname(__file__), "golden")
+
+
+def rel(a, b):
+    return float((a - b).norm() / b.norm().clamp_min(1e-20))
+
+
+def attention_case(ch=64, H=8, W=6, gamma=0.7, seed=0, B=2):
+    """blocks.Attention(ch, use_sn=False) in fp64 with weights drawn so that the logits are O(1)..O(3), an input x and
+    an upstream gradient."""
+    from cocosnet_b200.nets.blocks import Attention
+    g = torch.Generator().manual_seed(seed)
+    m = Attention(ch, False).double()
+    for conv in (m.theta, m.phi, m.g, m.o):
+        conv.weight.data.normal_(0, 1.0 / conv.in_channels ** 0.5, generator=g)
+    m.theta.weight.data *= 2.0
+    m.gamma.data.fill_(gamma)
+    x = torch.randn(B, ch, H, W, generator=g, dtype=torch.float64)
+    gy = torch.randn(B, ch, H, W, generator=g, dtype=torch.float64)
+    return m, x, gy
+
+
+def reference(m, x, gy):
+    """fp64 autograd through the mirror module (the reference's unfused bmm / softmax / bmm)."""
+    from oracle import torch_port
+    xr = x.clone().requires_grad_(True)
+    m.zero_grad(set_to_none=True)
+    with torch_port.cpu_reference_mode():
+        y = m(xr)
+    y.backward(gy)
+    return y.detach(), xr.grad, m.theta.weight.grad, m.phi.weight.grad, m.g.weight.grad, m.o.weight.grad, m.gamma.grad
+
+
+def on_the_tape(m, x, gy, mode=T.PRECISE, device="cpu"):
+    """tape.attention -> (y, dx, dtheta, dphi, dg, do, dgamma) as fp32 tensors on the CPU."""
+    ch, kd = x.shape[1], m.theta.out_channels
+
+    def body(tp, ins, params):
+        h = T.pack_in(tp, 0, ins[0], mode.raw, grad_ch=(0, ch))
+        return [T.unpack_out(tp, T.attention(tp, h, params[0], params[1], params[2], mode))]
+    f32 = lambda t: t.detach().float().to(device).clone().requires_grad_(True)  # noqa: E731
+    w_tpg = f32(torch.cat((m.theta.weight, m.phi.weight, m.g.weight), 0))
+    w_o, gam, xi = f32(m.o.weight), f32(m.gamma), f32(x)
+    y = T.run(body, [xi], [w_tpg, w_o, gam])[0]
+    y.backward(gy.float().to(device))
+    gt = w_tpg.grad.cpu()
+    return (y.detach().cpu(), xi.grad.cpu(), gt[:kd], gt[kd:2 * kd], gt[2 * kd:], w_o.grad.cpu(), gam.grad.cpu())
+
+
+@pytest.fixture(params=[True, False], ids=["exact", "rounded"])
+def emul(request):
+    old = nhwc.set_backend(AttnEmulBackend(exact=request.param))
+    yield request.param
+    nhwc.set_backend(old)
+
+
+NAMES = ("y", "x", "theta", "phi", "g", "o", "gamma")
+
+
+@pytest.mark.parametrize("shape", [(64, 8, 6), (128, 4, 12), (512, 4, 4)])  # 512: two stage-A chunks of 128
+def test_attention_matches_the_module_in_fp64(emul, shape):
+    ch, H, W = shape
+    m, x, gy = attention_case(ch, H, W)
+    want = reference(m, x, gy)
+    got = on_the_tape(m, x, gy)
+    # exact: every tensor fp32; rounded: fp16 operands (3-term split Q / K), bf16 gradients
+    tols = (2e-6, 5e-5, 5e-5, 5e-5, 5e-5, 5e-5, 5e-5) if emul else (2e-4, 1e-2, 2e-2, 2e-2, 1e-2, 1e-2, 1e-2)
+    for name, a, b, t in zip(NAMES, got, want, tols):
+        assert a.shape == b.shape, name
+        assert rel(a.double(), b) < t, (name, rel(a.double(), b))
+    # the block really attends: gamma * o(.) is a sizeable part of the output
+    assert float((want[0] - x).norm()) > 0.1 * float(x.norm())
+
+
+def test_attention_fast_mode_matches_the_module(emul):
+    m, x, gy = attention_case(64, 8, 8, seed=3)
+    want = reference(m, x, gy)
+    got = on_the_tape(m, x, gy, mode=T.FAST)
+    tols = (2e-6, 2e-5, 2e-5, 2e-5, 2e-5, 2e-5, 2e-5) if emul else (2e-3, 1e-2, 3e-2, 3e-2, 2e-2, 1e-2, 2e-2)
+    for name, a, b, t in zip(NAMES, got, want, tols):
+        assert rel(a.double(), b) < t, (name, rel(a.double(), b))
+
+
+def test_attention_at_gamma_zero(emul):
+    """At the initial gamma = 0 the block is the identity: the reference's gamma gradient <G, W_o> is nonzero and every
+    other weight gradient is exactly zero -- the tape must not form <gamma G, W_o> / gamma."""
+    m, x, gy = attention_case(64, 8, 6, gamma=0.0, seed=5)
+    want = reference(m, x, gy)
+    got = on_the_tape(m, x, gy)
+    assert torch.equal(got[0].double(), x.float().double())
+    assert rel(got[1].double(), gy) < (1e-6 if emul else 1e-2)
+    for name, a in zip(NAMES[2:6], got[2:6]):
+        assert torch.count_nonzero(a) == 0, name
+    for name, b in zip(NAMES[2:6], want[2:6]):
+        assert torch.count_nonzero(b) == 0, name
+    assert torch.isfinite(got[6]) and float(want[6].abs()) > 0
+    assert rel(got[6].double(), want[6]) < (2e-5 if emul else 1e-2)
+
+
+def test_pooling_argmax_routes_ties_like_max_pool2d():
+    """phi and g are max-pooled 2x2: with ties in a window the gradient goes to the first maximum in scan order, as
+    F.max_pool2d's backward does; the forward's pooled values are the window maxima."""
+    old = nhwc.set_backend(AttnEmulBackend(exact=True))
+    try:
+        import torch.nn.functional as F
+        B, H, W, kd, cv = 1, 4, 4, 8, 16
+        C = 2 * kd + cv
+        g = torch.Generator().manual_seed(2)
+        z = torch.randint(-2, 3, (B, C, H, W), generator=g).float()  # integers in [-2, 2]: many ties
+        z[:, :, :2, :2] = 1.0  # a window of four equal values
+        zr = z.clone().requires_grad_(True)
+        pooled = F.max_pool2d(zr[:, kd:], 2)
+        gp = torch.randn(pooled.shape, generator=g)
+        pooled.backward(gp)
+        zn = nhwc.pack(z, nhwc.F32)
+        q, k, vt, saved = nhwc.attn_pack(zn, kd, cv)
+        assert torch.equal(k[0, :, :kd], pooled[0, :kd].reshape(kd, -1).t())
+        assert torch.equal(vt[0, :cv, :4], pooled[0, kd:].reshape(cv, -1))
+        dq = torch.zeros(B, kd, H * W)
+        dk, dv = gp[:, :kd].reshape(B, kd, -1), gp[:, kd:].reshape(B, cv, -1)
+        dz = nhwc.new(B, H, W, C, nhwc.BF16, "cpu", zero=False)
+        nhwc.backend().attn_grad_unpack(dq, dk, dv, zn, kd, cv, dz)
+        assert torch.equal(dz.t[..., :C].permute(0, 3, 1, 2), zr.grad)
+        # the window of four equal values: everything to its top-left pixel
+        assert torch.equal(zr.grad[0, kd:, 0, 0], gp[0, :, 0, 0])
+        assert torch.count_nonzero(zr.grad[0, kd:, :2, :2].reshape(C - kd, 4)[:, 1:]) == 0
+    finally:
+        nhwc.set_backend(old)
+
+
+NONLOCAL_STEP_CASES = ["adaptor_nonlocal_dilation", "adaptor_nonlocal_gamma"]
+
+
+@pytest.mark.timeout(900)
+@pytest.mark.parametrize("name", NONLOCAL_STEP_CASES)
+def test_nonlocal_adaptor_step_on_the_tape_matches_reference_golden(name, monkeypatch):
+    """One generator + discriminator step at 64x64 with the --adaptor_nonlocal adaptor on the emulated tape (asserted:
+    every adaptor pass goes through fast.adaptor_forward and T.attention) against the golden of the unmodified
+    reference; the gamma case sets every Attention's gain to ATTN_GAMMA right after it is built, as its minting did."""
+    import tests.test_fast_path_cpu as tfp
+    from cocosnet_b200.nets import blocks, fast
+    from tests.golden.cases_attention import ATTENTION_CASES, set_gamma_on_construction
+    from tests.test_adaptor_variants_cpu import _compare_with_golden
+    from tests.golden.cases_small import SMALL_CASES
+    argv = ATTENTION_CASES.get(name) or SMALL_CASES[name]
+    taken, attended = [], []
+    real, real_attn = fast.adaptor_forward, T.attention
+
+    def counting(net, x, precise=True):
+        taken.append(type(net).__name__)
+        return real(net, x, precise)
+
+    def counting_attn(*a, **k):
+        attended.append(1)
+        return real_attn(*a, **k)
+    monkeypatch.setattr(fast, "adaptor_forward", counting)
+    monkeypatch.setattr(T, "attention", counting_attn)
+    monkeypatch.setattr(tfp, "EmulBackend", AttnEmulBackend)
+    if name in ATTENTION_CASES:
+        set_gamma_on_construction(blocks.Attention, monkeypatch.setattr)
+    got, grads = tfp._small_train_step(argv, fast=True)
+    assert len(taken) >= 2 and set(taken) == {"AdaptiveFeatureGenerator"}, taken
+    assert len(attended) == len(taken), (attended, taken)
+    gold = np.load(os.path.join(GOLD, "small_%s.npz" % name))
+    if name in ATTENTION_CASES:
+        extra = [k for k in gold.files if "attn." in k or "head_0.conv_1" in k]
+        assert len(extra) >= 10, extra
+    assert _compare_with_golden(name, got, grads) >= 10
