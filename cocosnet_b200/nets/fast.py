@@ -156,17 +156,9 @@ def spade_supported(norm):
     return (norm.pono or stat) and norm.mlp_gamma.kernel_size == (3, 3)
 
 
-def _wide_halos_and_se():
-    """Dilated blocks (reflection halos of 2 and 4 pixels) and squeeze-excitation need entry points a kernel emulation
-    may lack; the native backend has them."""
-    return getattr(nhwc.backend(), "wide_halos_and_se", False)
-
-
 def block_supported(blk):
     norms = [blk.norm_0, blk.norm_1] + ([blk.norm_s] if blk.learned_shortcut else [])
-    variant = blk.dilation != 1 or blk.use_se
-    return blk.dilation in (1, 2, 4) and (not variant or _wide_halos_and_se()) \
-        and all(spade_supported(n) for n in norms)
+    return blk.dilation in (1, 2, 4) and all(spade_supported(n) for n in norms)
 
 
 def register_block(ps, blk):
@@ -310,13 +302,12 @@ def _adaptor_blocks(net):
 
 def attention_supported(attn):
     """The SAGAN block on the tape (T.attention): four plain bias-free 1x1 convolutions without forward pre-hooks (no
-    spectral norm), at most 256 value channels (K1's limit), and a backend with the non-local entry points."""
+    spectral norm) and at most 256 value channels (K1's limit)."""
     convs = (attn.theta, attn.phi, attn.g, attn.o)
     plain = all(isinstance(c, nn.Conv2d) and c.kernel_size == (1, 1) and c.stride == (1, 1) and c.padding == (0, 0)
                 and c.dilation == (1, 1) and c.groups == 1 and c.bias is None and c.padding_mode == "zeros"
                 and not c._forward_pre_hooks for c in convs)
-    return plain and attn.theta.out_channels == attn.phi.out_channels and attn.g.out_channels <= 256 \
-        and getattr(nhwc.backend(), "nonlocal_attention", False)
+    return plain and attn.theta.out_channels == attn.phi.out_channels and attn.g.out_channels <= 256
 
 
 def adaptor_supported(net, x):

@@ -134,8 +134,6 @@ _DTYPES = {F16: torch.float16, BF16: torch.bfloat16, F32: torch.float32}
 class NativeBackend:
     """ctypes -> libcocos_b200.so.  No fallback: constructing it without the library raises."""
     exact = False
-    wide_halos_and_se = True  # reflection halos wider than one pixel (dilated SPADE blocks) and se_fwd / se_bwd
-    nonlocal_attention = True  # to_op, attn_pack / attn_do_rows / attn_grad_unpack and K1 / stage A / GEMM behind them
 
     def __init__(self):
         self.lib = _lib.lib()

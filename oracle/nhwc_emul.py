@@ -1,23 +1,27 @@
 """TEST INFRASTRUCTURE -- torch (CPU) emulation of the C-ABI entry points of the 16-bit NHWC pipeline
 (include/cocos_b200.h: cocos_tapconv, cocos_tapwgrad, cocos_pack_w, cocos_spade_mod_nhwc_*, cocos_in_stats_nhwc,
-cocos_inst_act_nhwc_*, cocos_nhwc_pack / unpack, cocos_colsum_nhwc), restating what each kernel computes from its
-descriptor -- including the TMA semantics the kernels rely on (zero fill outside the tensor, the parity-split view of
-stride-2 taps, the halo written by reflection from the epilogue).
+cocos_inst_act_nhwc_*, cocos_nhwc_pack / unpack, cocos_colsum_nhwc, cocos_se_nhwc_{fwd,bwd}, cocos_nhwc_to_op,
+cocos_attn_pack_nhwc, cocos_attn_do_rows, cocos_attn_grad_unpack, and K1 / its backward stage A / the GEMM behind
+tape.attention), restating what each kernel computes from its descriptor -- including the TMA semantics the kernels
+rely on (zero fill outside the tensor, the parity-split view of stride-2 taps, the reflection halo of any width
+p < H, W written from the epilogue).  It has every public method of the native backend.
 
 Only tests/ install it (cocosnet_b200.nhwc.set_backend): on CPU it checks the host-side planning (tap groups, weight
 layouts, halo / split bookkeeping, the hand-written backward formulas) against F.conv2d and autograd, and on the GPU
 it is the reference the kernels themselves are compared with.  `exact=True` keeps every tensor in fp32 (logic check
-at 1e-5); `exact=False` rounds to fp16 / bf16 where the kernels do.  The product never imports this module.
+at 1e-5); `exact=False` rounds to fp16 / bf16 where the kernels do.  K1 and stage A are emulated in fp32 in both
+modes (their own kernels are pinned by tests/test_gpu_corr.py).  The product never imports this module.
 """
 import torch
 
 F16, BF16, F32 = 1, 2, 3
 
 
-def _reflect_targets(idx, n):
-    """padded coordinates that hold a copy of interior index idx (pad 1): [self, mirror-low, mirror-high] masks."""
-    return [(idx + 1, torch.ones_like(idx, dtype=torch.bool)), (torch.zeros_like(idx), idx == 1),
-            (torch.full_like(idx, n + 1), idx == n - 2)]
+def _reflect_targets(idx, n, p):
+    """padded coordinates that hold a copy of interior index idx in a reflection halo of width p < n: [self,
+    mirror-low, mirror-high] with masks -- at most one mirror per side, as the tap-convolution epilogue stores them."""
+    return [(idx + p, torch.ones_like(idx, dtype=torch.bool)), (p - idx, (idx >= 1) & (idx <= p)),
+            (2 * (n - 1) - idx + p, (idx <= n - 2) & (idx >= n - 1 - p))]
 
 
 class EmulBackend:
@@ -95,8 +99,8 @@ class EmulBackend:
         p = d["y_pad"]
         co = d["y_coff"]
         hi = self._round(acc, d["y_kind"])
-        rts = _reflect_targets(yh, d["y_H"]) if (p and d["y_reflect"]) else [(yh + p, torch.ones_like(yh, dtype=torch.bool))]
-        cts = _reflect_targets(yw, d["y_W"]) if (p and d["y_reflect"]) else [(yw + p, torch.ones_like(yw, dtype=torch.bool))]
+        rts = _reflect_targets(yh, d["y_H"], p) if (p and d["y_reflect"]) else [(yh + p, torch.ones_like(yh, dtype=torch.bool))]
+        cts = _reflect_targets(yw, d["y_W"], p) if (p and d["y_reflect"]) else [(yw + p, torch.ones_like(yw, dtype=torch.bool))]
         for rt, rm in rts:
             for ct, cm in cts:
                 if not (rm.any() and cm.any()):
@@ -184,17 +188,19 @@ class EmulBackend:
 
     @staticmethod
     def _fold(t, pad):
-        """adjoint of _pad_reflect: [B,H+2p,W+2p,C] -> [B,H,W,C]."""
+        """adjoint of _pad_reflect (F.pad(mode="reflect")) for any pad < H, W: [B,H+2p,W+2p,C] -> [B,H,W,C]."""
         if not pad:
             return t
         t = t.clone()
-        H, W = t.shape[1] - 2, t.shape[2] - 2
-        t[:, 2] += t[:, 0]
-        t[:, H - 1] += t[:, H + 1]
-        t = t[:, 1:H + 1]
-        t[:, :, 2] += t[:, :, 0]
-        t[:, :, W - 1] += t[:, :, W + 1]
-        return t[:, :, 1:W + 1]
+        H, W = t.shape[1] - 2 * pad, t.shape[2] - 2 * pad
+        for k in range(1, pad + 1):  # halo row pad - k mirrors interior row k, halo row pad + H - 1 + k row H - 1 - k
+            t[:, pad + k] += t[:, pad - k]
+            t[:, pad + H - 1 - k] += t[:, pad + H - 1 + k]
+        t = t[:, pad:pad + H]
+        for k in range(1, pad + 1):
+            t[:, :, pad + k] += t[:, :, pad - k]
+            t[:, :, pad + W - 1 - k] += t[:, :, pad + W - 1 + k]
+        return t[:, :, pad:pad + W]
 
     def _write_op(self, y, val):
         """val fp32 [B,H,W,C] -> y (NT): hi (+ lo) with the reflection halo."""
@@ -363,3 +369,120 @@ class EmulBackend:
 
     def colsum(self, x, kind, Cs, C, rows, out):
         out[:C] = x.float().reshape(rows, Cs)[:, :C].sum(0)
+
+    # ---------------------------------------------------------------------------------------------- squeeze-excitation
+    def se_fwd(self, dx, res, w1, w2, y, m, hid, s):
+        C = dx.C
+        v = dx.t.float()[..., :C]
+        mm = v.mean((1, 2))
+        hh = (mm @ w1.float().t()).relu()
+        ss = torch.sigmoid(hh @ w2.float().t())
+        m.copy_(mm)
+        hid.copy_(hh)
+        s.copy_(ss)
+        y.t[..., :C] = (res.t.float()[..., :C] + ss[:, None, None, :] * v).to(y.t.dtype)
+
+    def se_bwd(self, dy, dx, w1, w2, m, hid, s, ddx, dw1, dw2):
+        C, hw = dx.C, dx.H * dx.W
+        v, g = dx.t.float()[..., :C], dy.t.float()[..., :C]
+        e2 = (v * g).sum((1, 2)) * s * (1 - s)           # d / d(pre-sigmoid)
+        e1 = (e2 @ w2.float()) * (hid > 0).float()        # d / d(pre-ReLU)
+        dm = e1 @ w1.float() / hw
+        dw1.copy_(e1.t() @ m)
+        dw2.copy_(e2.t() @ hid)
+        ddx.t[..., :C] = (s[:, None, None, :] * g + dm[:, None, None, :]).to(ddx.t.dtype)
+
+    # ---------------------------------------------------------------------------------------------- SAGAN attention
+    def _rows(self, v, kp, split, query):
+        """[B, N, kd] -> [B, N, kp * (3 if split else 1)]: [hi], or [hi, lo, hi] (query) / [hi, hi, lo] (key)."""
+        full = torch.zeros(v.shape[:2] + (kp,))
+        full[..., :v.shape[2]] = v
+        hi = self._round(full, F16)
+        if not split:
+            return hi
+        lo = self._round(full - hi, F16)
+        return torch.cat((hi, lo, hi) if query else (hi, hi, lo), 2)
+
+    def to_op(self, x, y):
+        v = x.t.float()
+        hi = self._round(v, F16)
+        y.t[..., :x.Cs] = hi.to(y.t.dtype)
+        if y.lo:
+            y.t[..., y.lo:y.lo + x.Cs] = self._round(v - hi, F16).to(y.t.dtype)
+
+    def attn_pack(self, z, kd, cv, split, q, k, vt, v16, q_cm, k_cm):
+        B, H, W = z.B, z.H, z.W
+        zf = z.t.float()
+        theta = zf[..., :kd].reshape(B, H * W, kd)
+        pooled = zf.reshape(B, H // 2, 2, W // 2, 2, zf.shape[3]).amax((2, 4)).reshape(B, H * W // 4, zf.shape[3])
+        phi, g = pooled[..., kd:2 * kd], pooled[..., 2 * kd:2 * kd + cv]
+        kp = q.shape[2] // (3 if split else 1)
+        q.copy_(self._rows(theta, kp, split, True).to(q.dtype))
+        k.copy_(self._rows(phi, kp, split, False).to(k.dtype))
+        nk = g.shape[1]
+        full = torch.zeros(vt.shape)
+        full[:, :cv, :nk] = g.transpose(1, 2)
+        vt.copy_(self._round(full, F16).to(vt.dtype))
+        if v16 is not None:  # [chunk, B, Nk, cvk]
+            nch, cvk = v16.shape[0], v16.shape[3]
+            full = torch.zeros(B, nk, nch * cvk)
+            full[..., :cv] = g
+            full = full.reshape(B, nk, nch, cvk).permute(2, 0, 1, 3)
+            v16.copy_(self._round(full, F16).to(v16.dtype))
+        if q_cm is not None:
+            q_cm.copy_(self._round(theta.transpose(1, 2), BF16).to(q_cm.dtype))
+            k_cm.copy_(self._round(phi.transpose(1, 2), BF16).to(k_cm.dtype))
+
+    @staticmethod
+    def _probs(q, k, lse=None):
+        s = q.float() @ k.float().transpose(1, 2)
+        if lse is None:
+            lse = torch.logsumexp(s, 2)
+        return torch.exp(s - lse[..., None]), lse
+
+    def attend_fwd(self, q, k, vt, cv, nk):
+        p, lse = self._probs(q, k)
+        out = (p @ vt.float()[:, :cv, :nk].transpose(1, 2)).transpose(1, 2).contiguous()
+        return out, lse
+
+    def attend_bwd_ds(self, q, k, do16, rscale, v16, out, lse, cv, want_pt=True):
+        p, _ = self._probs(q, k, lse)
+        do = do16.float()[..., :cv] / rscale[..., None]
+        dp = do @ v16.float()[..., :cv].transpose(1, 2)
+        ds = p * (dp - (do * out.transpose(1, 2)).sum(2, keepdim=True))
+        bf = lambda t: self._round(t, BF16).to(self.dtype(BF16))  # noqa: E731
+        return bf(ds), bf(ds.transpose(1, 2)), (bf(p.transpose(1, 2)) if want_pt else None)
+
+    def gemm(self, a, b, out=None):
+        c = a.float() @ b.float().transpose(1, 2)
+        return c if out is None else out.add_(c)
+
+    def attn_do_rows(self, dy, cv, do16, rscale, do_cm, out, out_ck):
+        B, N = dy.B, dy.H * dy.W
+        d = dy.t.float()[..., :cv].reshape(B, N, cv)
+        m = d.abs().amax(2)
+        r = torch.where((m > 0) & torch.isfinite(m), 1.0 / m, torch.ones_like(m))
+        rscale.copy_(r)
+        nch, cvk = do16.shape[0], do16.shape[3]
+        full = torch.zeros(B, N, nch * cvk)
+        full[..., :cv] = d * r[..., None]
+        do16.copy_(self._round(full.reshape(B, N, nch, cvk).permute(2, 0, 1, 3), F16).to(do16.dtype))
+        do_cm.copy_(d.transpose(1, 2).to(do_cm.dtype))
+        if out_ck is not None:  # chunk c: out[:, c*cvk : c*cvk + cv_c] as [B, cv_c, N] at offset c * B * cvk * N
+            for c in range(nch):
+                part = out[:, c * cvk:min(cv, (c + 1) * cvk)]
+                out_ck[c * B * cvk * N:][:part.numel()].copy_(part.reshape(-1))
+
+    def attn_grad_unpack(self, dq, dk, dv, z, kd, cv, dz):
+        B, H, W = z.B, z.H, z.W
+        c2 = kd + cv
+        out = torch.zeros(B, H, W, dz.Cs)
+        out[..., :kd] = dq.float().transpose(1, 2).reshape(B, H, W, kd)
+        win = z.t.float()[..., kd:kd + c2].reshape(B, H // 2, 2, W // 2, 2, c2).permute(0, 1, 3, 2, 4, 5) \
+            .reshape(B, H // 2, W // 2, 4, c2)
+        mx = win.max(3, keepdim=True).values
+        first = ((win == mx).cumsum(3) == 1) & (win == mx)  # the first maximum in scan order (F.max_pool2d's index)
+        g = torch.cat((dk.float(), dv.float()), 1).transpose(1, 2).reshape(B, H // 2, W // 2, 1, c2)
+        routed = torch.where(first, g, torch.zeros_like(g))
+        out[..., kd:kd + c2] = routed.reshape(B, H // 2, W // 2, 2, 2, c2).permute(0, 1, 3, 2, 4, 5).reshape(B, H, W, c2)
+        dz.t.copy_(out.to(dz.t.dtype))

@@ -9,7 +9,7 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
 from oracle import ref_harness as rh  # noqa: E402
-from tests.golden.cases_small import CROP, SMALL_CASES  # noqa: E402
+from tests.golden.cases_small import CONSTRUCTION_HOOKS, CROP, EXTRA_GRAD_KEYS, SMALL_CASES  # noqa: E402
 
 GRAD_KEYS = ("conv_img.weight", "theta.weight", "phi.weight", "layer1.0.weight_orig", "layer1.0.weight", "fc.weight",
              "attn.gamma", "layer.3.conv2.weight", "layer.0.prelu.weight", "up_3.norm_0.mlp_gamma.weight")
@@ -19,12 +19,20 @@ def run(name):
     from cocosnet_b200 import data as cdata
     from cocosnet_b200.options import TrainOptions
     argv = SMALL_CASES[name] + CROP
+    grad_keys = GRAD_KEYS + EXTRA_GRAD_KEYS.get(name, ())
     batch = cdata.synthetic_batch(TrainOptions().parse(argv + ["--gpu_ids", "-1"], save=False, verbose=False), 1)
     with rh.reference_imported(), rh.patched_for_cpu_training():
         opt = rh.make_opt(argv, True)
+        from models.networks import architecture
         from models.pix2pix_model import Pix2PixModel
-        torch.manual_seed(0)
-        model = Pix2PixModel(opt)
+        real_init = architecture.Attention.__init__
+        if name in CONSTRUCTION_HOOKS:
+            CONSTRUCTION_HOOKS[name](architecture.Attention)
+        try:
+            torch.manual_seed(0)
+            model = Pix2PixModel(opt)
+        finally:
+            architecture.Attention.__init__ = real_init  # the next case builds an unmodified model
         model.train()
 
         def fresh():
@@ -46,7 +54,7 @@ def run(name):
                     continue
                 net = model.net[key]
                 for pname, p in net.named_parameters():
-                    if p.grad is not None and pname.endswith(GRAD_KEYS):
+                    if p.grad is not None and pname.endswith(grad_keys):
                         res["gradnorm_%s_%s" % (key, pname)] = np.array([float(p.grad.norm())])
             d_losses = model(fresh(), mode="discriminator", GforD={"fake_image": out["fake_image"]})
             sum(d_losses.values()).mean().backward()

@@ -1,18 +1,13 @@
 """CPU: the SAGAN non-local block of the domain adaptor (--adaptor_nonlocal) on the NHWC tape -- tape.attention through
-the kernel emulation (tests/emul_attn.py) against the mirror module blocks.Attention in fp64 autograd, at gamma != 0
-and at the initial gamma = 0, the 2x2 argmax routing on ties, and the whole 64x64 training step of both
---adaptor_nonlocal flag sets against goldens minted from the unmodified reference."""
-import os
-
-import numpy as np
+the kernel emulation (oracle/nhwc_emul.py) against the mirror module blocks.Attention in fp64 autograd, at gamma != 0
+and at the initial gamma = 0, and the 2x2 argmax routing on ties.  The whole 64x64 training steps of both
+--adaptor_nonlocal flag sets against the goldens of the unmodified reference are in tests/test_fast_path_cpu.py."""
 import pytest
 import torch
 
 from cocosnet_b200 import nhwc
 from cocosnet_b200 import tape as T
-from tests.emul_attn import AttnEmulBackend
-
-GOLD = os.path.join(os.path.dirname(__file__), "golden")
+from oracle.nhwc_emul import EmulBackend
 
 
 def rel(a, b):
@@ -63,7 +58,7 @@ def on_the_tape(m, x, gy, mode=T.PRECISE, device="cpu"):
 
 @pytest.fixture(params=[True, False], ids=["exact", "rounded"])
 def emul(request):
-    old = nhwc.set_backend(AttnEmulBackend(exact=request.param))
+    old = nhwc.set_backend(EmulBackend(exact=request.param))
     yield request.param
     nhwc.set_backend(old)
 
@@ -114,7 +109,7 @@ def test_attention_at_gamma_zero(emul):
 def test_pooling_argmax_routes_ties_like_max_pool2d():
     """phi and g are max-pooled 2x2: with ties in a window the gradient goes to the first maximum in scan order, as
     F.max_pool2d's backward does; the forward's pooled values are the window maxima."""
-    old = nhwc.set_backend(AttnEmulBackend(exact=True))
+    old = nhwc.set_backend(EmulBackend(exact=True))
     try:
         import torch.nn.functional as F
         B, H, W, kd, cv = 1, 4, 4, 8, 16
@@ -140,43 +135,3 @@ def test_pooling_argmax_routes_ties_like_max_pool2d():
         assert torch.count_nonzero(zr.grad[0, kd:, :2, :2].reshape(C - kd, 4)[:, 1:]) == 0
     finally:
         nhwc.set_backend(old)
-
-
-NONLOCAL_STEP_CASES = ["adaptor_nonlocal_dilation", "adaptor_nonlocal_gamma"]
-
-
-@pytest.mark.timeout(900)
-@pytest.mark.parametrize("name", NONLOCAL_STEP_CASES)
-def test_nonlocal_adaptor_step_on_the_tape_matches_reference_golden(name, monkeypatch):
-    """One generator + discriminator step at 64x64 with the --adaptor_nonlocal adaptor on the emulated tape (asserted:
-    every adaptor pass goes through fast.adaptor_forward and T.attention) against the golden of the unmodified
-    reference; the gamma case sets every Attention's gain to ATTN_GAMMA right after it is built, as its minting did."""
-    import tests.test_fast_path_cpu as tfp
-    from cocosnet_b200.nets import blocks, fast
-    from tests.golden.cases_attention import ATTENTION_CASES, set_gamma_on_construction
-    from tests.test_adaptor_variants_cpu import _compare_with_golden
-    from tests.golden.cases_small import SMALL_CASES
-    argv = ATTENTION_CASES.get(name) or SMALL_CASES[name]
-    taken, attended = [], []
-    real, real_attn = fast.adaptor_forward, T.attention
-
-    def counting(net, x, precise=True):
-        taken.append(type(net).__name__)
-        return real(net, x, precise)
-
-    def counting_attn(*a, **k):
-        attended.append(1)
-        return real_attn(*a, **k)
-    monkeypatch.setattr(fast, "adaptor_forward", counting)
-    monkeypatch.setattr(T, "attention", counting_attn)
-    monkeypatch.setattr(tfp, "EmulBackend", AttnEmulBackend)
-    if name in ATTENTION_CASES:
-        set_gamma_on_construction(blocks.Attention, monkeypatch.setattr)
-    got, grads = tfp._small_train_step(argv, fast=True)
-    assert len(taken) >= 2 and set(taken) == {"AdaptiveFeatureGenerator"}, taken
-    assert len(attended) == len(taken), (attended, taken)
-    gold = np.load(os.path.join(GOLD, "small_%s.npz" % name))
-    if name in ATTENTION_CASES:
-        extra = [k for k in gold.files if "attn." in k or "head_0.conv_1" in k]
-        assert len(extra) >= 10, extra
-    assert _compare_with_golden(name, got, grads) >= 10

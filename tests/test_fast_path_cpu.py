@@ -1,7 +1,7 @@
-"""CPU: the 16-bit NHWC tape (cocosnet_b200/tape.py, nets/fast.py) -- generator, domain adaptors, residual stack,
-discriminators, VGG -- driven through the torch emulation of the kernels (oracle/nhwc_emul.py, exact mode) must
-reproduce the goldens minted from the unmodified reference: same losses, outputs and gradient norms as the plain
-host mirror.  This pins the host side of the fast path (tape bookkeeping, hand-written backward chain, weight
+"""CPU: the 16-bit NHWC tape (cocosnet_b200/tape.py, nets/fast.py) -- generator, domain adaptors and their variants,
+residual stack, discriminators, VGG -- driven through the torch emulation of the kernels (oracle/nhwc_emul.py, exact
+mode) must reproduce the goldens minted from the unmodified reference: same losses, outputs and gradient norms as the
+plain host mirror.  This pins the host side of the fast path (tape bookkeeping, hand-written backward chain, weight
 gathering incl. spectral norm) to the reference without a GPU; the kernels are pinned to the emulation on the GPU."""
 import os
 
@@ -151,25 +151,53 @@ def _small_train_step(argv, fast, crop=64):
     return vals, grads
 
 
-from tests.golden.cases_small import EXTENDED_ONLY, SMALL_CASES  # noqa: E402
+from tests.golden.cases_small import CONSTRUCTION_HOOKS, EXTENDED_ONLY, EXTRA_GRAD_KEYS, SMALL_CASES  # noqa: E402
 
-_SMALL_RUN = [n for n in SMALL_CASES if os.environ.get("COCOS_ALL_SMALL_CASES") == "1" or n not in EXTENDED_ONLY]
+_ALL = os.environ.get("COCOS_ALL_SMALL_CASES") == "1"
+_ADAPTOR_VARIANTS = ("--adaptor_se", "--adaptor_res_deeper", "--dilation_conv", "--adaptor_nonlocal")
+_VARIANT_CASES = [n for n in SMALL_CASES if any(f in SMALL_CASES[n] for f in _ADAPTOR_VARIANTS)]
+# every case through the dispatch a GPU run does; with COCOS_ALL_SMALL_CASES=1 also the adaptor-variant cases a second
+# time on the mirror modules (COCOS_NHWC=0), which the tape has replaced for them
+_SMALL_RUN = [pytest.param(n, True, id=n) for n in SMALL_CASES if _ALL or n not in EXTENDED_ONLY] + \
+    [pytest.param(n, False, id=n + "-modules") for n in _VARIANT_CASES if _ALL]
 
 
-@pytest.mark.timeout(600)
-@pytest.mark.parametrize("name", _SMALL_RUN)
-def test_small_flag_sets_match_reference_golden(name):
-    """11 more flag sets (17 with COCOS_ALL_SMALL_CASES=1: + the variants whose layers the tape does not take) at 64x64 against goldens minted from the UNMODIFIED reference (tests/golden/
-    make_golden_small.py): the option branches the three 256x256 goldens do not reach -- odd channel counts in the
-    residual stack (--use_coordconv 409, celebahq / deepfashion + --maskmix 275 / 276: C % 8 in 1..4 needs zero-filled
-    channel slots), the column-softmax mask, both cycle terms, the other GAN modes, adaptor variants, D_cam ...  Run with
-    the tape on the kernel emulation: whatever the tape supports runs on it, the rest on the mirror modules -- exactly
-    the dispatch a GPU run does.  Losses / outputs to fp32 rounding; gradient norms to 2e-2: 1/T = 100 amplifies fp32
-    rounding into the correspondence gradients, and at this size the REFERENCE's own fp32 gradients are the noisy side --
-    against an fp64 evaluation of the same step (match_kernel_1) the reference / mirror arithmetic is off by 1.2e-2 on
-    the PReLU slopes and 1e-3 on theta / phi, the tape by 3e-4 / 1e-5 (its convolutions accumulate in a different order)."""
+@pytest.mark.timeout(900)
+@pytest.mark.parametrize("name,fast", _SMALL_RUN)
+def test_small_flag_sets_match_reference_golden(name, fast, monkeypatch):
+    """15 more flag sets (19 with COCOS_ALL_SMALL_CASES=1: + the ones whose layers the tape does not take, and then the
+    four adaptor-variant cases once more on the mirror modules) at 64x64 against goldens minted from the UNMODIFIED
+    reference (tests/golden/make_golden_small.py): the option branches the
+    three 256x256 goldens do not reach -- odd channel counts in the residual stack (--use_coordconv 409, celebahq /
+    deepfashion + --maskmix 275 / 276: C % 8 in 1..4 needs zero-filled channel slots), the column-softmax mask, both cycle
+    terms, the other GAN modes, adaptor variants, D_cam ...  Run with the tape on the kernel emulation: whatever the tape
+    supports runs on it, the rest on the mirror modules -- exactly the dispatch a GPU run does.  The adaptor-variant cases
+    assert that every adaptor pass took the tape (and T.attention with --adaptor_nonlocal).  Losses / outputs to fp32
+    rounding; gradient norms to 2e-2: 1/T = 100 amplifies fp32 rounding into the correspondence gradients, and at this
+    size the REFERENCE's own fp32 gradients are the noisy side -- against an fp64 evaluation of the same step
+    (match_kernel_1) the reference / mirror arithmetic is off by 1.2e-2 on the PReLU slopes and 1e-3 on theta / phi, the
+    tape by 3e-4 / 1e-5 (its convolutions accumulate in a different order)."""
+    from cocosnet_b200 import tape as T
+    from cocosnet_b200.nets import blocks
+    from cocosnet_b200.nets import fast as fast_nets
+    taken, attended = [], []
+    real_adaptor, real_attention = fast_nets.adaptor_forward, T.attention
+    monkeypatch.setattr(fast_nets, "adaptor_forward",
+                        lambda net, x, precise=True: taken.append(type(net).__name__) or real_adaptor(net, x, precise))
+    monkeypatch.setattr(T, "attention", lambda *a, **k: attended.append(1) or real_attention(*a, **k))
+    if name in CONSTRUCTION_HOOKS:
+        CONSTRUCTION_HOOKS[name](blocks.Attention, monkeypatch.setattr)
     gold = np.load(os.path.join(GOLD, "small_%s.npz" % name))
-    got, grads = _small_train_step(SMALL_CASES[name], fast=True)
+    got, grads = _small_train_step(SMALL_CASES[name], fast=fast)
+    if name in _VARIANT_CASES and fast:
+        assert len(taken) >= 2 and set(taken) == {"AdaptiveFeatureGenerator"}, taken
+        if "--adaptor_nonlocal" in SMALL_CASES[name]:
+            assert len(attended) == len(taken), (attended, taken)
+    if not fast:
+        assert not taken and not attended, (taken, attended)
+    # the case's extra gradient norms are in its golden, for both adaptors
+    extra = [k for k in gold.files if k.startswith("gradnorm_") and k.endswith(EXTRA_GRAD_KEYS.get(name, ()))]
+    assert len(extra) >= 2 * len(EXTRA_GRAD_KEYS.get(name, ())), extra
     for key in gold.files:
         if key.startswith(("g_", "d_")):
             assert np.allclose(got[key].numpy(), gold[key], rtol=5e-4, atol=2e-6), (key, got[key], gold[key])

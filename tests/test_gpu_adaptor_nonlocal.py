@@ -1,42 +1,19 @@
 """GPU: the SAGAN non-local block of the domain adaptor (--adaptor_nonlocal) on the NHWC tape -- the four new kernels
 (cocos_nhwc_to_op, cocos_attn_pack_nhwc, cocos_attn_do_rows, cocos_attn_grad_unpack) against their CPU emulation
-(tests/emul_attn.py, pinned to autograd by tests/test_adaptor_nonlocal_cpu.py), tape.attention against fp64 autograd
-through the mirror module at the adaptor, generator and discriminator shapes, repeatability, both 64x64 training steps
-against the goldens of the unmodified reference, and a CUDA-graph replay with every adaptor variant."""
-import copy
-import os
-
-import numpy as np
+(oracle/nhwc_emul.py, pinned to autograd by tests/test_adaptor_nonlocal_cpu.py), tape.attention against fp64 autograd
+through the mirror module at the adaptor, generator and discriminator shapes, repeatability, and a CUDA-graph replay
+with every adaptor variant.  Both 64x64 --adaptor_nonlocal training steps against the goldens of the unmodified
+reference are in tests/test_gpu_adaptor_variants.py."""
 import pytest
 import torch
 
 from cocosnet_b200 import nhwc
-from cocosnet_b200 import tape as T
-from tests.emul_attn import AttnEmulBackend
+from tests.harness import both, graph_replay_vs_eager, rel
 from tests.test_adaptor_nonlocal_cpu import attention_case, on_the_tape, reference
 
 pytestmark = pytest.mark.gpu
 
-GOLD = os.path.join(os.path.dirname(__file__), "golden")
 _ADE = ["--dataset_mode", "ade20k", "--PONO", "--PONO_C"]
-
-
-def rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    assert torch.isfinite(a).all(), "non-finite values in the kernel output"
-    return float((a - b).norm() / b.norm().clamp_min(1e-30))
-
-
-def both(fn):
-    """fn(device) -> tuple of tensors; returns (native on cuda, rounded emulation on cpu)."""
-    old = nhwc.set_backend(AttnEmulBackend(exact=False))
-    try:
-        want = fn("cpu")
-    finally:
-        nhwc.set_backend(old)
-    got = fn("cuda")
-    torch.cuda.synchronize()
-    return [t.cpu() for t in got], want
 
 
 # Nk = 64, 1024, 4096 (features 16^2, 64^2, 128^2) x Cv = 128, 256 (ch = 256, 512: Kd = 32, 64)
@@ -83,6 +60,7 @@ def test_new_kernels_match_their_emulation(h, cv):
     assert len(got) == len(want)
     for i, (a, b) in enumerate(zip(got, want)):
         assert a.shape == b.shape, (i, a.shape, b.shape)
+        a = a.cpu()
         assert torch.equal(a.float(), b.float()), (i, float((a.float() - b.float()).abs().max()))
 
 
@@ -121,107 +99,11 @@ def test_attention_at_gamma_zero_on_the_gpu():
     assert rel(got[6], want[6]) < 5e-2, rel(got[6], want[6])
 
 
-def _small_model(argv, seed=0):
-    from tests.test_gpu_adaptor_variants import _small_model as sm
-    return sm(argv, seed)
-
-
-@pytest.mark.timeout(900)
-@pytest.mark.parametrize("name", ["adaptor_nonlocal_dilation", "adaptor_nonlocal_gamma"])
-def test_nonlocal_adaptor_step_matches_reference_golden(name, monkeypatch):
-    """The default path (--conv_precision split) with the adaptor's SAGAN block on the tape against the 64x64 goldens:
-    1e-3 on warp_out and fake_image, the losses and gradient norms as tests/test_gpu_adaptor_variants.py checks them."""
-    from cocosnet_b200 import data as cdata
-    from cocosnet_b200.nets import blocks
-    from tests.golden.cases_attention import ATTENTION_CASES, set_gamma_on_construction
-    from tests.golden.cases_small import SMALL_CASES
-    from tests.test_gpu_adaptor_variants import _Without
-    from tests.test_gpu_model import _check_losses_and_grads, _rel
-    taken = []
-    real_attn = T.attention
-    monkeypatch.setattr(T, "attention", lambda *a, **k: taken.append(1) or real_attn(*a, **k))
-    if name in ATTENTION_CASES:
-        set_gamma_on_construction(blocks.Attention, monkeypatch.setattr)
-    gold = np.load(os.path.join(GOLD, "small_%s.npz" % name))
-    opt, model = _small_model(ATTENTION_CASES.get(name) or SMALL_CASES[name])
-    batch = cdata.synthetic_batch(opt, 1)
-    g_losses, out = model(batch, mode="generator")
-    sum(g_losses.values()).mean().backward()
-    d_losses = model(batch, mode="discriminator", GforD={"fake_image": out["fake_image"]})
-    assert len(taken) >= 2  # both adaptor passes ran the block on the tape
-    warp = _rel(out["warp_out"].detach().cpu().numpy()[:, :, ::2, ::2], gold["warp_out_sub"])
-    fake = _rel(out["fake_image"].detach().cpu().numpy()[:, :, ::2, ::2], gold["fake_image_sub"])
-    print(name, "warp_out %.2e fake_image %.2e" % (warp, fake))
-    assert warp < 1e-3, warp
-    assert fake < 1e-3, fake
-    # scalar parameters: one big cancelling sum each.  PReLU slopes 15 % as in test_gpu_adaptor_variants.py.  The
-    # gain's gradient <G, W_o> sums B*H*W*512*256 products of the bf16 gradient and the bf16 copy of o's input and is
-    # 1e-4..1e-7 of their magnitude here: on an H100 (700 W) it came out 82 % (gamma = 0) and 28 % (gamma = 300) off
-    # the golden, so only its order of magnitude is checked on the GPU; tests/test_adaptor_nonlocal_cpu.py holds it
-    # to 5 % on the exact tape, and the gamma != 0 block test above to 5 % against fp64 at O(1) gradients.
-    params = {k: dict(model.net[k].named_parameters()) for k in ("netG", "netCorr", "netD")}
-    scalar = [k for k in gold.files if k.startswith("gradnorm_")
-              and params[k.split("_", 2)[1]][k.split("_", 2)[2]].numel() <= 16]
-    _check_losses_and_grads(model, _Without(gold, scalar), g_losses, d_losses, out, 1.0)
-    for key in scalar:
-        _, netk, pname = key.split("_", 2)
-        have, want = float(params[netk][pname].grad.norm()), float(gold[key][0])
-        if pname.endswith("attn.gamma"):
-            assert want / 3 <= have <= 3 * want, (key, have, want)
-        else:
-            assert abs(have - want) <= 0.15 * want + 1e-7, (key, have, want)
-
-
 @pytest.mark.timeout(900)
 def test_graph_replay_equals_eager_step_with_the_nonlocal_adaptor():
     """trainer.run_step with --adaptor_nonlocal --adaptor_se --adaptor_res_deeper --dilation_conv (64x64, batch 2): the
     replayed CUDA graph and an eager step from the same snapshot give the same losses and parameter updates."""
-    from cocosnet_b200 import data as cdata
-    from cocosnet_b200.options import TrainOptions
-    from cocosnet_b200.trainer import Pix2PixTrainer
-    from oracle import torch_port
-
-    if os.environ.get("COCOS_CUDA_GRAPH", "1") != "1":
-        pytest.skip("CUDA-graph step disabled by COCOS_CUDA_GRAPH=0")
     flags = ["--adaptor_nonlocal", "--adaptor_se", "--adaptor_res_deeper", "--dilation_conv"]
-
-    def make(use_graph):
-        opt = TrainOptions().parse(_ADE + flags + ["--crop_size", "64", "--load_size", "64", "--batchSize", "2",
-                                                   "--gpu_ids", "0"], save=False, verbose=False)
-        opt.verbose_networks = False
-        opt.allow_random_vgg = True
-        torch.manual_seed(0)
-        trainer = Pix2PixTrainer(opt)
-        trainer.pix2pix_model.vggnet_fix.load_state_dict(torch_port.seeded_vgg_state_dict())
-        if not use_graph:
-            trainer.graph_error = "disabled for the comparison"
-        return opt, trainer
-
-    opt, tg = make(True)
-    for it in range(tg.GRAPH_WARMUP):
-        tg.run_step(cdata.synthetic_batch(opt, 2, seed=100 + it))
-    torch.cuda.synchronize()
-    snap = {"model": copy.deepcopy(tg.pix2pix_model.state_dict()), "G": copy.deepcopy(tg.optimizer_G.state_dict()),
-            "D": copy.deepcopy(tg.optimizer_D.state_dict())}
-    batch = cdata.synthetic_batch(opt, 2, seed=777)
-    tg.run_step(batch)
-    assert tg._graph is not None, tg.graph_error
-    lg = {k: float(v.mean()) for k, v in tg.get_latest_losses().items()}
-    _, te = make(False)
-    te.pix2pix_model.load_state_dict(snap["model"])
-    te.optimizer_G.load_state_dict(snap["G"])
-    te.optimizer_D.load_state_dict(snap["D"])
-    te.run_step(batch)
-    le = {k: float(v.mean()) for k, v in te.get_latest_losses().items()}
-    for k in le:
-        assert abs(lg[k] - le[k]) <= 2e-3 * max(abs(le[k]), 1.0), (k, lg[k], le[k])
-    pg, pe = dict(tg.pix2pix_model.named_parameters()), dict(te.pix2pix_model.named_parameters())
-    names = [n for n in pe if "adaptive_model_seg" in n and any(s in n for s in (
-        "attn.theta.weight", "attn.g.weight", "attn.o.weight", "attn.gamma", "head_0.se_layar.fc.0.weight"))]
-    assert len(names) == 5, names
-    for name in names:
-        before = snap["model"][name].float()
-        ug, ue = pg[name].detach().float() - before, pe[name].detach().float() - before
-        assert float(ue.norm()) > 0, name
-        cos = float((ug * ue).sum() / (ug.norm() * ue.norm()))
-        assert cos > 0.99, (name, cos)
+    seg = "net.netCorr.adaptive_model_seg."
+    graph_replay_vs_eager(_ADE + flags + ["--crop_size", "64", "--load_size", "64"], 2, [seg + n for n in (
+        "attn.theta.weight", "attn.g.weight", "attn.o.weight", "attn.gamma", "head_0.se_layar.fc.0.weight")])

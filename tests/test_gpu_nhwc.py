@@ -7,26 +7,9 @@ import torch
 
 from cocosnet_b200 import nhwc
 from oracle.nhwc_emul import EmulBackend
+from tests.harness import both, rel
 
 pytestmark = pytest.mark.gpu
-
-
-def rel(a, b):
-    a, b = a.float().cpu(), b.float().cpu()
-    assert torch.isfinite(a).all(), "non-finite values in the kernel output"
-    return float((a - b).norm() / b.norm().clamp_min(1e-20))
-
-
-def both(fn):
-    """fn(device) -> tuple of tensors; returns (native on cuda, emulation on cpu)."""
-    old = nhwc.set_backend(EmulBackend(exact=False))
-    try:
-        want = fn("cpu")
-    finally:
-        nhwc.set_backend(old)
-    got = fn("cuda")
-    torch.cuda.synchronize()
-    return got, want
 
 
 def make(case, seed=0):

@@ -180,6 +180,14 @@ def test_plan_dgrad_covers_every_tap_once():
         assert sorted(taps) == sorted(itertools.product(range(ks), range(ks)))
 
 
+def test_emulation_has_every_public_method_of_the_native_backend():
+    """The tape never asks a backend what it supports: whatever the native backend offers, the emulation has too.
+    Compared on the class (constructing NativeBackend loads the library)."""
+    public = {n for n in vars(nhwc.NativeBackend) if not n.startswith("_")}
+    missing = public - set(dir(EmulBackend(exact=True)))
+    assert not missing, sorted(missing)
+
+
 def test_bench_tapconv_roofline_bookkeeping_on_the_emulation():
     """bench.py's `roofline_tapconv` object: the launch it times is the one nhwc.conv plans (1 MMA term per tap for
     single operands, 3 for 2-term split operands), and its FLOP accounting is 2*B*H*W*Cout*Cin*9 per launch."""

@@ -12,6 +12,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 from cocosnet_b200 import data as cdata  # noqa: E402
 import test_gpu_model as G  # noqa: E402
+from tests import harness as H  # noqa: E402
 import test_model_parity_cpu as M  # noqa: E402
 
 
@@ -22,7 +23,7 @@ def rel(a, b):
 
 def train(config):
     gold = np.load(os.path.join(G.GOLD, "model_%s.npz" % config))
-    opt, model = G._build(gpu=True, config=config)
+    opt, model = H.build_model(G.MODEL_CONFIGS[config])
     batch = cdata.synthetic_batch(opt, 1)
     g_losses, out = model(batch, mode="generator")
     sum(g_losses.values()).mean().backward()

@@ -11,6 +11,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 from cocosnet_b200 import data as cdata  # noqa: E402
 import test_gpu_model as G  # noqa: E402
+from tests import harness as H  # noqa: E402
 
 
 def rel(a, b):
@@ -44,7 +45,7 @@ def main():
     outs = {}
     seen = None
     for gpu in (False, True):
-        opt, model = G._build(gpu=gpu, config=config)
+        opt, model = H.build_model(G.MODEL_CONFIGS[config], gpu=gpu)
         batch = cdata.synthetic_batch(opt, 1)
         grab = {}
         corr = model.net["netCorr"]
