@@ -1,7 +1,14 @@
-"""Synthetic data provider with the reference's batch-dict schema
-(data/pix2pix_dataset.py:138-144): label, image, ref, label_ref, self_ref, path.
-Real dataset readers (PIL/cv2 preprocessing) are out of scope (SURVEY.md 2.1 #11).
+"""Data for train.py / test.py, in the reference's batch-dict schema (data/pix2pix_dataset.py:138-144): label, image,
+ref, label_ref, self_ref, path.
+
+create_dataloader reads the real ADE20k, CelebA-HQ and DeepFashion datasets (cocosnet_b200/datasets.py) when
+--dataroot is an existing directory.  Otherwise -- and for celebahqedge, flickr and synthetic, which have no reader --
+it serves SyntheticDataset: blocky random label maps and uniform-noise images, which is also what bench.py and the
+tests feed the model (synthetic_batch).
 """
+import os
+import random
+
 import numpy as np
 import torch
 import torch.utils.data
@@ -59,11 +66,24 @@ def synthetic_batch(opt, batch, seed=1234, pin=False):
 def create_dataloader(opt, seed=0):
     """Global batches of opt.batchSize (data/__init__.py:40-60).  The shuffle order comes from a generator seeded
     identically on every rank, so with one process per GPU all ranks draw the SAME global batch and
-    trainer.shard_batch() hands each its contiguous slice -- DataParallel.scatter's split of one batch."""
-    ds = SyntheticDataset(opt)
-    print("dataset [%s] of size %d was created" % (type(ds).__name__, len(ds)))
+    trainer.shard_batch() hands each its contiguous slice -- DataParallel.scatter's split of one batch.
+
+    A real reader (when opt.dataroot is a directory and the mode has one) decodes in opt.nThreads workers.  Its
+    random draws (crops, flips, references) then agree on every rank too: the DataLoader seeds each worker's `random`
+    from the same generator, and this process's `random` -- which the DeepFashion reference lists draw from while they
+    are read, and which serves every item when opt.nThreads is 0 -- is seeded from `seed` before the reader is built.
+    The synthetic data is generated in the main process from per-item seeds."""
+    from .datasets import READERS
     gen = torch.Generator()
     gen.manual_seed(seed)
+    if opt.dataset_mode in READERS and os.path.isdir(opt.dataroot):
+        random.seed(seed)
+        ds = READERS[opt.dataset_mode](opt)
+        print("dataset [%s] of size %d was created" % (type(ds).__name__, len(ds)))
+        return torch.utils.data.DataLoader(ds, batch_size=opt.batchSize, shuffle=not opt.serial_batches,
+                                           num_workers=int(opt.nThreads), drop_last=opt.isTrain, generator=gen)
+    ds = SyntheticDataset(opt)
+    print("dataset [%s] of size %d was created" % (type(ds).__name__, len(ds)))
     return torch.utils.data.DataLoader(ds, batch_size=opt.batchSize, shuffle=not opt.serial_batches,
                                        num_workers=0, drop_last=opt.isTrain, generator=gen)
 
