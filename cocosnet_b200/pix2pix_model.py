@@ -22,6 +22,8 @@ class Pix2PixModel(torch.nn.Module):
         self.opt = opt
         self.alpha = 1
         self.after_netG_backward = None  # trainer hook: called once the backward has left netG (its gradients are final)
+        self.free_inference_graph()
+        self.infer_graph_error = None
         self.net = torch.nn.ModuleDict(self.initialize_networks(opt))
         if opt.isTrain:
             self.vggnet_fix = networks.VGG19_feature_color_torchversion(vgg_normal_correct=opt.vgg_normal_correct)
@@ -67,6 +69,91 @@ class Pix2PixModel(torch.nn.Module):
             out["ref_semantics"] = ref_semantics
             return out
         raise ValueError("|mode| is invalid")
+
+    # ------------------------------------------------------------------ CUDA-graph inference
+    def run_inference(self, data):
+        """`self(data, mode="inference")`, replayed from one CUDA graph: the same keys and the same bits.  On a CUDA
+        model in eval() the first call for an input signature (the batch's shapes plus the identity and address of
+        every parameter and buffer of netG and netCorr) runs eagerly as warm-up, the next call with that signature
+        captures the forward, and from then on a call copies the batch into static device buffers and replays the
+        graph: one launch in place of the forward's per-op dispatch.  One signature is kept: a batch of other shapes
+        (test.py's short last batch) runs eagerly.  Weights updated in place (load_state_dict, an optimiser step) are
+        read by the replay; replacing a parameter tensor re-captures.
+        Eager always on the CPU, in train(), under COCOS_CUDA_GRAPH=0, and with --noise_for_mask / --mask_noise,
+        whose random draws a replay would not repeat.  The returned tensors are copies: a later call does not
+        overwrite them."""
+        self.check_glasses_slot(data)  # the capture skips preprocess_input's host-side assertion: check it here
+        if not self.inference_graph_capable():
+            return self(data, mode="inference")
+        shapes = tuple((k, tuple(v.shape), v.dtype) for k, v in sorted(data.items()) if torch.is_tensor(v))
+        key = (shapes, self._weights_key())
+        if self._infer["graph"] is not None and key != self._infer["key"]:
+            if shapes != self._infer["key"][0]:
+                return self(data, mode="inference")  # not the captured shapes
+            self.free_inference_graph()  # a parameter or buffer was replaced: warm up and capture again
+        if self._infer["graph"] is None:
+            if key != self._infer["warm_key"]:
+                self._infer["warm_key"] = key
+                return self(data, mode="inference")
+            self._capture_inference(data, key)
+            if self._infer["graph"] is None:  # capture failed: stay eager, loudly
+                return self(data, mode="inference")
+        g = self._infer
+        for k, buf in g["static_in"].items():
+            buf.copy_(data[k], non_blocking=True)
+        g["graph"].replay()
+        return {k: (v.clone() if torch.is_tensor(v) else v) for k, v in g["static_out"].items()}
+
+    def inference_graph_capable(self):
+        opt = self.opt
+        return (not self.training and next(self.net["netG"].parameters()).is_cuda and self.use_gpu()
+                and os.environ.get("COCOS_CUDA_GRAPH", "1") == "1" and self.infer_graph_error is None
+                and not getattr(opt, "noise_for_mask", False) and not getattr(opt, "mask_noise", False))
+
+    def free_inference_graph(self):
+        """Drop the captured inference forward and its private memory pool."""
+        self._infer = {"graph": None, "key": None, "warm_key": None, "static_in": None, "static_out": None}
+
+    def _weights_key(self):
+        nets = (self.net["netG"], self.net["netCorr"])
+        return tuple((id(t), t.data_ptr()) for n in nets for t in list(n.parameters()) + list(n.buffers()))
+
+    def _capture_inference(self, data, key):
+        from . import nhwc
+        static_in = {k: torch.empty_like(v, device="cuda") for k, v in data.items() if torch.is_tensor(v)}
+        for k, buf in static_in.items():
+            buf.copy_(data[k], non_blocking=True)
+        static = dict(data)
+        static.update(static_in)
+        torch.cuda.synchronize()
+        graph = torch.cuda.CUDAGraph()
+        # everything the graph reads must be produced inside it (or be immutable): the weight packs are re-made by
+        # every replay from the parameters' storage, which is what makes in-place weight updates visible to it
+        nhwc.clear_pack_cache()
+        try:
+            with torch.no_grad(), torch.cuda.graph(graph):  # captured on torch.cuda.graph's side stream
+                out = self(static, mode="inference")
+        except Exception as e:  # noqa: BLE001 -- an op that cannot be captured: report it and keep running eagerly
+            self.infer_graph_error = "%s: %s" % (type(e).__name__, str(e).splitlines()[0] if str(e) else "")
+            print("cocosnet_b200: CUDA-graph capture of inference failed (%s); running eagerly" % self.infer_graph_error)
+            if os.environ.get("COCOS_GRAPH_TRACE", "0") == "1":
+                import traceback
+                traceback.print_exc()
+            torch.cuda.synchronize()
+            nhwc.clear_pack_cache()
+            return
+        nhwc.clear_pack_cache()  # buffers packed during the capture live in the graph's pool: not for eager use
+        self._infer = {"graph": graph, "key": key, "warm_key": None, "static_in": static_in, "static_out": out}
+
+    def check_glasses_slot(self, data):
+        """celebahq: preprocess_input's assertion that no pixel has the id of the glasses slot (semantic_nc - 3, which
+        the glasses channel fills), on the host batch -- a captured forward cannot run it, so run_inference does it on
+        every path before the batch reaches the GPU.  Raises the same AssertionError."""
+        if self.opt.dataset_mode != "celebahq":
+            return
+        slot = self.opt.semantic_nc - 3
+        assert not bool((data["label"][:, ::2].long() == slot).any())
+        assert not bool((data["label_ref"][:, ::2].long() == slot).any())
 
     def create_optimizers(self, opt):
         G_params = [{"params": self.net["netG"].parameters(), "lr": opt.lr * 0.5},
