@@ -181,7 +181,7 @@ __global__ void __launch_bounds__(256) attn_kv_kernel(const AttnPack p) {
 
 // ----------------------------------------------------------------------------------------------- dO rows
 // dy bf16 [B, N, dy_Cs] (Cv channels) -> do16 fp16 [nchunk, B, N, Cvk] = r * dy in chunks of Cvk channels (zero beyond
-// Cv), r = 1 / max_c |dy| (1 for an all-zero row), do_cm bf16 [B, Cv, Nqp] = dy channel-major and, with more than one
+// Cv), r = min(1 / max_c |dy|, 2^126) (1 for an all-zero row), do_cm bf16 [B, Cv, Nqp] = dy channel-major and, with more than one
 // chunk, out_ck = K1's output out fp32 [B, Cv, N] regrouped per chunk ([B, cv_chunk, N] each).  32 positions per block,
 // one warp per row for the maxima.
 __global__ void __launch_bounds__(256)
@@ -202,7 +202,8 @@ attn_do_rows_kernel(const uint16_t* __restrict__ dy, int dy_Cs, int N, int Cv, u
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
     if (tx == 0) {
-      const float r = (m > 0.f && isfinite(m)) ? 1.0f / m : 1.0f;
+      // capped at 2^126: 1/m overflows fp32 for a subnormal maximum m <= 2^-128 (rowscale_kernel in pack.cu)
+      const float r = (m > 0.f && isfinite(m)) ? fminf(1.0f / m, 0x1p126f) : 1.0f;
       rs[i] = r;
       if (n < N) rscale[static_cast<size_t>(b) * N + n] = r;
     }

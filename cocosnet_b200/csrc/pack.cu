@@ -85,7 +85,7 @@ pack_v_kernel(const float* __restrict__ src, uint16_t* __restrict__ dst, int Cv,
   dst[(static_cast<size_t>(b) * Cvp + c) * Nkp + n] = bits;
 }
 
-// r[b,n] = 1 / max_c |src[b,c,n]|  (1 where the column is all zero)
+// r[b,n] = min(1 / max_c |src[b,c,n]|, 2^126)  (1 where the column is all zero)
 __global__ void __launch_bounds__(256)
 rowscale_kernel(const float* __restrict__ src, float* __restrict__ r, int C, int N) {
   const int b = blockIdx.y;
@@ -94,7 +94,9 @@ rowscale_kernel(const float* __restrict__ src, float* __restrict__ r, int C, int
   const float* s = src + static_cast<size_t>(b) * C * N + n;
   float m = 0.f;
   for (int c = 0; c < C; ++c) m = fmaxf(m, fabsf(s[static_cast<size_t>(c) * N]));
-  r[static_cast<size_t>(b) * N + n] = (m > 0.f && isfinite(m)) ? 1.0f / m : 1.0f;
+  // 1/m overflows fp32 for a subnormal m <= 2^-128: cap r at 2^126 so that r * x stays <= 1 and the divide-back
+  // (scale / r in stage A) stays finite; every normal m keeps r = 1/m exactly
+  r[static_cast<size_t>(b) * N + n] = (m > 0.f && isfinite(m)) ? fminf(1.0f / m, 0x1p126f) : 1.0f;
 }
 
 }  // namespace

@@ -36,7 +36,7 @@ def round_up(x, m):
 
 def pack_rows(x, kp=None, split=0, rowscale=False, bf16=False):
     """fp32 [B,C,N] -> fp16 [B,N,Kt] (see cocos_pack_rows_f16).  With rowscale=True every
-    position is scaled by r = 1/max_c|x| first and (packed, r [B,N]) is returned."""
+    position is scaled by r = min(1/max_c|x|, 2^126) first and (packed, r [B,N]) is returned."""
     _req(x, torch.float32, "x")
     b, c, n = x.shape
     kp = round_up(c, 64) if kp is None else kp

@@ -39,7 +39,7 @@ const char* cocos_last_error(void);
  * operand rounding.  split_mode: 0 = plain fp16; 1 = query side [hi, lo, hi];
  * 2 = key side [hi, hi, lo] (one GEMM then sums hi*hi + lo*hi + hi*lo); 4 = plain bf16 instead of fp16.
  * rowscale_out (may be NULL): if given, every position n is first multiplied by
- * r[b,n] = 1 / max_c |src[b,c,n]| and r is written to rowscale_out [B,N] (used for
+ * r[b,n] = min(1 / max_c |src[b,c,n]|, 2^126) and r is written to rowscale_out [B,N] (used for
  * the upstream gradient dO in the backward so it always fits fp16). */
 int cocos_pack_rows_f16(const float* src, void* dst, int B, int C, int N, int Kp, int split_mode, float* rowscale_out,
                         void* stream);
@@ -402,7 +402,7 @@ int cocos_attn_pack_nhwc(const void* z, int z_kind, int z_Cs, int B, int H, int 
                          void* stream);
 /* dO rows of the attend backward from dy, the bf16 NHWC gradient of the attention output ([B, N, dy_Cs], Cv channels;
  * the gradient of bmm(g, beta^T) in architecture.py:126): do16 fp16 [ceil(Cv / Cvk), B, N, Cvk] = r * dy in chunks of
- * Cvk channels (Cvk % 64 == 0, zero beyond Cv) with r = 1 / max_c |dy| over all Cv channels (1 for an all-zero row)
+ * Cvk channels (Cvk % 64 == 0, zero beyond Cv) with r = min(1 / max_c |dy|, 2^126) over all Cv channels (1 for an all-zero row)
  * written to rscale [B, N] -- what cocos_pack_rows_f16 with rowscale_out makes from fp32 channel-major -- and do_cm
  * bf16 [B, Cv, Nqp] = dy channel-major, the A operand of the dV GEMM.  With more than one chunk, out_chunks receives
  * K1's output out fp32 [B, Cv, N] regrouped per chunk (chunk c: [B, cv_c, N] at offset c * B * Cvk * N), the `out`

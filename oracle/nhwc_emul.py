@@ -461,7 +461,8 @@ class EmulBackend:
         B, N = dy.B, dy.H * dy.W
         d = dy.t.float()[..., :cv].reshape(B, N, cv)
         m = d.abs().amax(2)
-        r = torch.where((m > 0) & torch.isfinite(m), 1.0 / m, torch.ones_like(m))
+        # capped at 2^126 like the kernel: 1/m overflows fp32 for a subnormal maximum m <= 2^-128
+        r = torch.where((m > 0) & torch.isfinite(m), (1.0 / m).clamp_max(2.0 ** 126), torch.ones_like(m))
         rscale.copy_(r)
         nch, cvk = do16.shape[0], do16.shape[3]
         full = torch.zeros(B, N, nch * cvk)

@@ -106,6 +106,23 @@ def test_attention_at_gamma_zero(emul):
     assert rel(got[6].double(), want[6]) < (2e-5 if emul else 1e-2)
 
 
+def test_attention_backward_with_a_subnormal_gradient_row(emul):
+    """The attend backward scales every dO row by r = 1 / max_c |dO| before the fp16 cast and divides r back out of
+    dS.  For a row whose maximum is subnormal (<= 2^-128), 1/m overflows fp32: uncapped, that query row of dS became
+    NaN, and through the dK GEMM (which reads it as a column of dS^T) so did every element of dphi.  r is capped at
+    2^126, so every gradient stays finite and within the usual bars of fp64 autograd."""
+    m, x, gy = attention_case(64, 8, 8, seed=11, B=1)
+    gy[0, :, 2, 3] *= 1e-39  # the attention output's gradient at that pixel: gamma * W_o^T gy, max ~1e-39 < 2^-128
+    want = reference(m, x, gy)
+    got = on_the_tape(m, x, gy)
+    # the bars of test_attention_matches_the_module_in_fp64, but 2e-2 on the gain's gradient (one cancelling sum: 1.2e-2
+    # off fp64 at this seed with the row left at its normal scale, too), as in test_attention_fast_mode_matches_the_module
+    tols = (2e-6, 5e-5, 5e-5, 5e-5, 5e-5, 5e-5, 5e-5) if emul else (2e-4, 1e-2, 2e-2, 2e-2, 1e-2, 1e-2, 2e-2)
+    for name, a, b, t in zip(NAMES, got, want, tols):
+        assert torch.isfinite(a).all(), (name, int((~torch.isfinite(a)).sum()), "non-finite elements")
+        assert rel(a.double(), b) < t, (name, rel(a.double(), b))
+
+
 def test_pooling_argmax_routes_ties_like_max_pool2d():
     """phi and g are max-pooled 2x2: with ties in a window the gradient goes to the first maximum in scan order, as
     F.max_pool2d's backward does; the forward's pooled values are the window maxima."""

@@ -30,6 +30,9 @@ def test_new_kernels_match_their_emulation(h, cv):
     z[:, ::3, :, 1::2] = z[:, ::3, :, 0::2]  # every 2x2 window of a third of the channels has a tied maximum
     dy = torch.randn(B, cv, h, h, generator=g) * torch.logspace(-3, 3, h * h).reshape(1, 1, h, h)  # rows of any scale
     dy[0, :, 0, 0] = 0  # an all-zero row: scale 1
+    # rows with a subnormal maximum: ~1.5e-39 (1/m overflows fp32) and ~5e-39 (1/m finite, above 2^126): both r = 2^126
+    dy[1, :, 0, 1] = torch.linspace(-1.5e-39, 1.5e-39, cv)
+    dy[1, :, 0, 2] = torch.linspace(-5e-39, 2e-39, cv)
     dq = torch.randn(B, kd, h * h, generator=g)
     dk, dv = torch.randn(B, kd, h * h // 4, generator=g), torch.randn(B, cv, h * h // 4, generator=g)
     out = torch.randn(B, cv, h * h, generator=g)  # K1's output, regrouped per stage-A chunk

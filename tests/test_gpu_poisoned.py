@@ -9,8 +9,9 @@ torch.utils.deterministic.fill_uninitialized_memory every one of them starts as 
 NaN in an output, a loss or a gradient.
 
 The module runs, under that poisoning:
-  * the per-kernel tests of test_gpu_nhwc.py, test_gpu_corr.py and the kernel-level tests of test_gpu_adaptor_variants.py
-    and test_gpu_adaptor_nonlocal.py, imported here so that pytest collects them once more in this module;
+  * the per-kernel tests of test_gpu_nhwc.py, test_gpu_corr.py, test_gpu_attend_edges.py and the kernel-level tests of
+    test_gpu_adaptor_variants.py and test_gpu_adaptor_nonlocal.py, imported here so that pytest collects them once more
+    in this module;
   * the channel widths whose storage has slots nobody computes -- C % 8 in 1..4, where the norm / activation kernels
     write round_up(C, 4) channels of round_up(C, 8) (3, 275, 276, 409) and C = 5, odd but without such a gap -- through
     every NHWC op with that rule or that writes padding slots, against the emulation, with the padding slots required
@@ -84,6 +85,9 @@ from tests.test_gpu_adaptor_variants import (  # noqa: E402,F401
     test_wide_halos_through_every_writer_and_fold)
 from tests.test_gpu_adaptor_nonlocal import (  # noqa: E402,F401
     test_attention_at_gamma_zero_on_the_gpu, test_attention_matches_fp64_autograd, test_new_kernels_match_their_emulation)
+from tests.test_gpu_attend_edges import (  # noqa: E402,F401
+    test_corr_attend_forward_backward_per_element, test_gemm_per_element, test_k1_forward_per_element,
+    test_nhwc_attend_two_stage_a_chunks_per_element, test_stage_a_per_element)
 from tests.test_gpu_model import test_train_step_matches_reference_golden  # noqa: E402,F401
 
 
