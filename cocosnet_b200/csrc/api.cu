@@ -20,6 +20,7 @@ int cocos_pack_v_f16(const float* src, void* dst, int B, int Cv, int Nk, int Cvp
   return pack_v_f16_launch(src, dst, B, Cv, Nk, Cvp, Nkp, bf16, static_cast<cudaStream_t>(stream));
 }
 
+// any Cvp % 16 == 0: beyond 256 value rows K1 runs in chunks of 256 (corr_fwd.cu)
 int cocos_corr_warp_fwd(const void* q, const void* k, const void* vt, const float* v32, float* out, float* lse,
                         float* corr, int B, int Nq, int Nk, int Kd, int Cv, int Cvp, int Nkp, float scale,
                         void* stream) {
@@ -42,6 +43,7 @@ int cocos_gemm_f16(const void* a, const void* b, float* c, int batch, int M, int
                          bf16, static_cast<cudaStream_t>(stream));
 }
 
+// any Cvk % 64 == 0: dO / V resident up to 192 channels, streamed through the operand ring beyond (corr_bwd.cu)
 int cocos_corr_warp_bwd_ds(const void* q, const void* k, const void* do16, const void* v16, const float* rscale,
                            const float* out, const float* lse, void* ds, void* dst, void* pt, int B, int Nq, int Nk,
                            int Kd, int Cv, int Cvk, int Nkp, int Nqp, float scale, void* stream) {

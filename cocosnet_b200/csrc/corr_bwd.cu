@@ -12,6 +12,11 @@
 // CTA = 128 query rows, streams 128-key tiles.  warp 8: TMA, warps 0-7: two
 // warpgroups of 64 query rows; S and dP by wgmma into registers, the softmax
 // Jacobian on the accumulator fragments, dS staged through one smem tile.
+//
+// Two shared-memory plans.  Resident (Cvk <= 192): the CTA's dO tile stays in smem, each key tile's V tile is loaded
+// whole.  Streamed (Cvk > 192, where dO + V no longer fit beside a 2-stage ring): the 64-channel atoms of dO and V go
+// through the same ring as the Q / K atoms, [dO atom | V atom] after the tile's [Q atom | K atom] stages, and
+// dP = dO V^T is a longer wgmma K loop accumulated in registers.  dS, dS^T and P^T are written once per tile either way.
 #include "corr_kernels.h"
 #include "ptx.cuh"
 #include "tmap.h"
@@ -26,7 +31,8 @@ constexpr int BM = 128, BN = 128, BK = 64;
 constexpr int ATOM_BYTES = 128 * BK * 2;
 constexpr int NUM_THREADS = 32 * CONSUMER_WARPS + 32;
 constexpr int CT = 32 * CONSUMER_WARPS;  // consumer threads
-constexpr int MAX_STAGES = 4;
+constexpr int MAX_STAGES = 5;
+constexpr int MAX_RESIDENT_STAGES = 4;
 constexpr int TPITCH = 136;                     // staging tile pitch (fp16 elements)
 constexpr int TILE_BYTES = 128 * TPITCH * 2;    // 34816
 
@@ -74,6 +80,8 @@ __device__ __forceinline__ void copy_tile_out(const uint8_t* tile, uint16_t* gba
   }
 }
 
+// STREAM: the streamed plan (dO / V atoms through the ring) instead of the resident one
+template <bool STREAM>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 corr_bwd_ds_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
                    const __grid_constant__ CUtensorMap tm_do, const __grid_constant__ CUtensorMap tm_v,
@@ -86,8 +94,8 @@ corr_bwd_ds_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
   const int q0 = blockIdx.x * BM, bidx = blockIdx.y;
   const int T = p.n_tiles;
 
-  const uint32_t stage_bytes = 2 * ATOM_BYTES;                 // [Q chunk | K chunk]
-  const uint32_t op_bytes = p.vc_count * ATOM_BYTES;           // dO tile / V tile
+  const uint32_t stage_bytes = 2 * ATOM_BYTES;                 // [Q chunk | K chunk] (streamed: or [dO | V])
+  const uint32_t op_bytes = STREAM ? 0 : p.vc_count * ATOM_BYTES;  // resident dO tile / V tile
   const uint32_t k_ring = smem0;
   const uint32_t do_smem = k_ring + p.ns * stage_bytes;
   const uint32_t v_smem = do_smem + op_bytes;
@@ -115,9 +123,11 @@ corr_bwd_ds_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
 
   if (warp == CONSUMER_WARPS) {
     if (lane == 0) {
-      mbar_expect_tx(smem_u32(&bars->do_full), op_bytes);
-      for (int vc = 0; vc < p.vc_count; ++vc)
-        tma_load_3d(do_smem + vc * ATOM_BYTES, &tm_do, smem_u32(&bars->do_full), vc * BK, q0, bidx);
+      if constexpr (!STREAM) {
+        mbar_expect_tx(smem_u32(&bars->do_full), op_bytes);
+        for (int vc = 0; vc < p.vc_count; ++vc)
+          tma_load_3d(do_smem + vc * ATOM_BYTES, &tm_do, smem_u32(&bars->do_full), vc * BK, q0, bidx);
+      }
       uint32_t ks = 0, kph = 0;
       for (int j = 0; j < T; ++j) {
         for (int kc = 0; kc < p.kc_count; ++kc) {
@@ -128,10 +138,21 @@ corr_bwd_ds_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
           tma_load_3d(k_ring + ks * stage_bytes + ATOM_BYTES, &tm_k, full, kc * BK, j * BN, bidx);
           if (++ks == static_cast<uint32_t>(p.ns)) { ks = 0; kph ^= 1; }
         }
-        mbar_wait(smem_u32(&bars->v_empty), (j & 1) ^ 1);
-        mbar_expect_tx(smem_u32(&bars->v_full), op_bytes);
-        for (int vc = 0; vc < p.vc_count; ++vc)
-          tma_load_3d(v_smem + vc * ATOM_BYTES, &tm_v, smem_u32(&bars->v_full), vc * BK, j * BN, bidx);
+        if constexpr (STREAM) {
+          for (int vc = 0; vc < p.vc_count; ++vc) {
+            mbar_wait(smem_u32(&bars->k_empty[ks]), kph ^ 1);
+            const uint32_t full = smem_u32(&bars->k_full[ks]);
+            mbar_expect_tx(full, stage_bytes);
+            tma_load_3d(k_ring + ks * stage_bytes, &tm_do, full, vc * BK, q0, bidx);
+            tma_load_3d(k_ring + ks * stage_bytes + ATOM_BYTES, &tm_v, full, vc * BK, j * BN, bidx);
+            if (++ks == static_cast<uint32_t>(p.ns)) { ks = 0; kph ^= 1; }
+          }
+        } else {
+          mbar_wait(smem_u32(&bars->v_empty), (j & 1) ^ 1);
+          mbar_expect_tx(smem_u32(&bars->v_full), op_bytes);
+          for (int vc = 0; vc < p.vc_count; ++vc)
+            tma_load_3d(v_smem + vc * ATOM_BYTES, &tm_v, smem_u32(&bars->v_full), vc * BK, j * BN, bidx);
+        }
       }
     }
     __syncwarp();
@@ -159,7 +180,7 @@ corr_bwd_ds_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
     }
   }
   const int valid_rows = min(BM, p.Nq - q0);
-  mbar_wait(smem_u32(&bars->do_full), 0);
+  if constexpr (!STREAM) mbar_wait(smem_u32(&bars->do_full), 0);
 
   uint32_t ks = 0, kph = 0;
   for (int j = 0; j < T; ++j) {
@@ -179,18 +200,36 @@ corr_bwd_ds_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
       if (lane == 0) mbar_arrive(smem_u32(&bars->k_empty[ks]));
       if (++ks == static_cast<uint32_t>(p.ns)) { ks = 0; kph ^= 1; }
     }
-    mbar_wait_quiet(smem_u32(&bars->v_full), j & 1);
-    wgmma_fence();
-    for (int vc = 0; vc < p.vc_count; ++vc) {
+    if constexpr (STREAM) {
+      for (int vc = 0; vc < p.vc_count; ++vc) {
+        mbar_wait_quiet(smem_u32(&bars->k_full[ks]), kph);
+        const uint32_t st = k_ring + ks * stage_bytes;
+        wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < 4; ++k)
-        wgmma_ss<BN, false>(dp, desc_advance_k16(make_desc_k_sw128(do_smem + vc * ATOM_BYTES + a_off), k),
-                            desc_advance_k16(make_desc_k_sw128(v_smem + vc * ATOM_BYTES), k), (vc | k) != 0 ? 1 : 0, 0);
+        for (int k = 0; k < 4; ++k)
+          wgmma_ss<BN, false>(dp, desc_advance_k16(make_desc_k_sw128(st + a_off), k),
+                              desc_advance_k16(make_desc_k_sw128(st + ATOM_BYTES), k), (vc | k) != 0 ? 1 : 0, 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(smem_u32(&bars->k_empty[ks]));
+        if (++ks == static_cast<uint32_t>(p.ns)) { ks = 0; kph ^= 1; }
+      }
+    } else {
+      mbar_wait_quiet(smem_u32(&bars->v_full), j & 1);
+      wgmma_fence();
+      for (int vc = 0; vc < p.vc_count; ++vc) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          wgmma_ss<BN, false>(dp, desc_advance_k16(make_desc_k_sw128(do_smem + vc * ATOM_BYTES + a_off), k),
+                              desc_advance_k16(make_desc_k_sw128(v_smem + vc * ATOM_BYTES), k), (vc | k) != 0 ? 1 : 0,
+                              0);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(smem_u32(&bars->v_empty));
     }
-    wgmma_commit();
-    wgmma_wait<0>();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(smem_u32(&bars->v_empty));
 
     // fragment element i: row r0 + 8 * ((i >> 1) & 1), column 8 * (i >> 2) + cq + (i & 1)
     uint32_t dsp[BN / 4];  // bf16 pairs (i, i + 1) for even i
@@ -262,10 +301,13 @@ int corr_bwd_ds_launch(const void* q, const void* k, const void* do16, const voi
   p.scale = scale; p.scale_log2 = scale * 1.4426950408889634f;
   p.do16 = static_cast<const __half*>(do16); p.rscale = rscale; p.out = out; p.lse = lse;
   p.ds = static_cast<uint16_t*>(ds); p.dst = static_cast<uint16_t*>(dst); p.pt = static_cast<uint16_t*>(pt);
+  // resident plan up to Cvk = 192 (dO and V tiles beside a ring of >= 2 stages); streamed beyond, where the ring
+  // also carries the dO / V atoms and its depth no longer depends on Cvk
+  const bool stream_vo = Cvk > 192;
   const int budget = 227 * 1024 - 1024 - 512;
-  const int fixed = 2 * p.vc_count * ATOM_BYTES + TILE_BYTES;
+  const int fixed = (stream_vo ? 0 : 2 * p.vc_count * ATOM_BYTES) + TILE_BYTES;
   p.ns = (budget - fixed) / (2 * ATOM_BYTES);
-  if (p.ns > MAX_STAGES) p.ns = MAX_STAGES;
+  if (p.ns > (stream_vo ? MAX_STAGES : MAX_RESIDENT_STAGES)) p.ns = stream_vo ? MAX_STAGES : MAX_RESIDENT_STAGES;
   if (p.ns < 2) {
     set_error("corr_bwd_ds: shared memory plan failed (Cvk=%d)", Cvk);
     return -1;
@@ -279,10 +321,10 @@ int corr_bwd_ds_launch(const void* q, const void* k, const void* do16, const voi
     return rc;
   if ((rc = make_tmap_f16_3d(&tm_v, v16, Cvk, Nk, B, (uint64_t)Cvk * 2, (uint64_t)Nk * Cvk * 2, BK, BN, 1)))
     return rc;
-  COCOS_CUDA_CHECK(
-      cudaFuncSetAttribute(corr_bwd_ds_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+  auto kernel = stream_vo ? corr_bwd_ds_kernel<true> : corr_bwd_ds_kernel<false>;
+  COCOS_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
   dim3 grid((Nq + BM - 1) / BM, B);
-  corr_bwd_ds_kernel<<<grid, NUM_THREADS, smem_bytes, stream>>>(tm_q, tm_k, tm_do, tm_v, p);
+  kernel<<<grid, NUM_THREADS, smem_bytes, stream>>>(tm_q, tm_k, tm_do, tm_v, p);
   COCOS_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

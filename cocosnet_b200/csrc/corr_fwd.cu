@@ -13,6 +13,9 @@
 //              * PVN > 0: O += P V by wgmma with P as the fp16 register operand (O in registers, N = PVN >= Cvp);
 //              * CV > 0 (Cv <= 4 value channels, fp32 V): P V on the CUDA cores inside the exp loop, P and V stay
 //                fp32 (no fp16 rounding of the probabilities).
+// More than 256 padded value channels (a TMA box and a wgmma N stop at 256): V is split into chunks of 256 rows along
+// grid z, each CTA recomputes S and the online softmax for its chunk, and a second launch takes a partial last chunk
+// with the PVN that fits it.  lse (and the raw logits) come from chunk 0 only.
 #include "corr_kernels.h"
 #include "ptx.cuh"
 #include "tmap.h"
@@ -31,6 +34,7 @@ constexpr int K_ATOM = BN * BK * 2;  // 8 KiB: 64 rows x 64 fp16
 constexpr int NUM_THREADS = 32 * CONSUMER_WARPS + 32;
 constexpr int MAX_KSTAGES = 8;
 constexpr int MAX_VSTAGES = 2;
+constexpr int VCHUNK = 256;  // value rows per chunk: the TMA box limit and the widest wgmma N
 
 struct FwdParams {
   int B, Nq, Nk, Kd, Cv, Cvp;
@@ -39,6 +43,8 @@ struct FwdParams {
   int q_resident;  // Q tile kept in smem for the whole CTA
   int ns_k, ns_v;
   int v_stage;     // bytes per V stage
+  int v_rows;      // value rows per chunk (the V box), <= PVN
+  int c0;          // first value row of chunk blockIdx.z == 0; chunk z starts at c0 + z * VCHUNK
   float scale, scale_log2;
   float* out;   // [B, Cv, Nq]
   float* lse;   // [B, Nq] (natural log) or null
@@ -77,6 +83,7 @@ corr_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   const int lane = tid & 31;
   const int q0 = blockIdx.x * BM;
   const int bidx = blockIdx.y;
+  const int cbase = p.c0 + blockIdx.z * VCHUNK;
 
   const uint32_t stage_bytes = p.q_resident ? K_ATOM : Q_ATOM + K_ATOM;
   const uint32_t q_smem = smem0;
@@ -113,7 +120,7 @@ corr_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         for (int kc = 0; kc < p.kc_count; ++kc)
           tma_load_3d(q_smem + kc * Q_ATOM, &tm_q, smem_u32(&bars->q_full), kc * BK, q0, bidx);
       }
-      const uint32_t v_bytes = PVN ? static_cast<uint32_t>(p.Cvp) * BN * 2 : static_cast<uint32_t>(CV) * BN * 4;
+      const uint32_t v_bytes = PVN ? static_cast<uint32_t>(p.v_rows) * BN * 2 : static_cast<uint32_t>(CV) * BN * 4;
       uint32_t ks = 0, kph = 0, vs = 0, vph = 0;
       for (int j = 0; j < T; ++j) {
         for (int kc = 0; kc < p.kc_count; ++kc) {
@@ -131,7 +138,7 @@ corr_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         mbar_wait(smem_u32(&bars->v_empty[vs]), vph ^ 1);
         const uint32_t vfull = smem_u32(&bars->v_full[vs]);
         mbar_expect_tx(vfull, v_bytes);
-        tma_load_3d(v_ring + vs * p.v_stage, &tm_v, vfull, j * BN, 0, bidx);
+        tma_load_3d(v_ring + vs * p.v_stage, &tm_v, vfull, j * BN, cbase, bidx);
         if (++vs == static_cast<uint32_t>(p.ns_v)) { vs = 0; vph ^= 1; }
       }
     }
@@ -177,7 +184,7 @@ corr_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     }
 
     const int kbase = j * BN + cq;
-    if (p.corr != nullptr) {
+    if (p.corr != nullptr && cbase == 0) {
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) {
         const int q = q0 + r0 + ((i >> 1) & 1) * 8, key = kbase + 8 * (i >> 2) + (i & 1);
@@ -255,7 +262,7 @@ corr_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 #pragma unroll
         for (int i = 0; i < ON; ++i) {
           if (((i >> 1) & 1) != r) continue;
-          const int c = 8 * (i >> 2) + cq + (i & 1);
+          const int c = cbase + 8 * (i >> 2) + cq + (i & 1);
           if (c < p.Cv) p.out[(static_cast<size_t>(bidx) * p.Cv + c) * p.Nq + q] = o[i] * inv_l;
         }
       }
@@ -266,20 +273,55 @@ corr_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         if (q < p.Nq && (t & 3) == c) p.out[(static_cast<size_t>(bidx) * p.Cv + c) * p.Nq + q] = v * inv_l;
       }
     }
-    if (p.lse != nullptr && q < p.Nq && (t & 3) == 0)
+    if (p.lse != nullptr && cbase == 0 && q < p.Nq && (t & 3) == 0)
       p.lse[static_cast<size_t>(bidx) * p.Nq + q] = (m[r] * c2 + log2f(lt)) * 0.6931471805599453f;
   }
 }
 
 template <int PVN, int CV>
 int launch_fwd(const CUtensorMap& tm_q, const CUtensorMap& tm_k, const CUtensorMap& tm_v, const FwdParams& p,
-               int smem_bytes, cudaStream_t stream) {
+               int smem_bytes, cudaStream_t stream, int n_chunks = 1) {
   COCOS_CUDA_CHECK(
       cudaFuncSetAttribute(corr_fwd_kernel<PVN, CV>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-  dim3 grid((p.Nq + BM - 1) / BM, p.B);
+  dim3 grid((p.Nq + BM - 1) / BM, p.B, n_chunks);
   corr_fwd_kernel<PVN, CV><<<grid, NUM_THREADS, smem_bytes, stream>>>(tm_q, tm_k, tm_v, p);
   COCOS_CUDA_CHECK(cudaGetLastError());
   return 0;
+}
+
+// shared memory plan (<= 227 KiB): [Q] [K ring] [V ring] [barriers]; sets q_resident / ns_k / ns_v from p.v_stage
+int plan_smem(FwdParams& p) {
+  const int budget = 227 * 1024 - 1024 /*alignment slack*/ - 512 /*barriers*/;
+  p.q_resident = (p.Kd <= 256) ? 1 : 0;
+  const int q_bytes = p.q_resident ? p.kc_count * Q_ATOM : 0;
+  const int stage = p.q_resident ? K_ATOM : Q_ATOM + K_ATOM;
+  p.ns_v = 2;
+  p.ns_k = (budget - q_bytes - p.ns_v * p.v_stage) / stage;
+  if (p.ns_k > MAX_KSTAGES) p.ns_k = MAX_KSTAGES;
+  if (p.ns_k < 2) {
+    set_error("corr_warp_fwd: shared memory plan failed (Kd=%d Cvp=%d)", p.Kd, p.Cvp);
+    return -1;
+  }
+  return 1024 + q_bytes + p.ns_k * stage + p.ns_v * p.v_stage + 512;
+}
+
+// tensor-core P V over n_chunks chunks of `rows` value rows, the first at row c0
+int launch_tensor_pv(const CUtensorMap& tm_q, const CUtensorMap& tm_k, const void* vt, FwdParams p, int Nkp, int rows,
+                     int c0, int n_chunks, cudaStream_t stream) {
+  const int pvn = rows <= 64 ? 64 : rows <= 128 ? 128 : 256;
+  // a V stage holds PVN rows of 64 keys (the wgmma reads PVN >= rows rows)
+  p.v_stage = pvn * BN * 2;
+  p.v_rows = rows;
+  p.c0 = c0;
+  const int smem_bytes = plan_smem(p);
+  if (smem_bytes < 0) return -1;
+  CUtensorMap tm_v;
+  int rc;
+  if ((rc = make_tmap_f16_3d(&tm_v, vt, p.Nk, p.Cvp, p.B, (uint64_t)Nkp * 2, (uint64_t)p.Cvp * Nkp * 2, BK, rows, 1)))
+    return rc;
+  if (pvn == 64) return launch_fwd<64, 0>(tm_q, tm_k, tm_v, p, smem_bytes, stream, n_chunks);
+  if (pvn == 128) return launch_fwd<128, 0>(tm_q, tm_k, tm_v, p, smem_bytes, stream, n_chunks);
+  return launch_fwd<256, 0>(tm_q, tm_k, tm_v, p, smem_bytes, stream, n_chunks);
 }
 
 }  // namespace
@@ -303,8 +345,12 @@ int corr_warp_fwd_launch(const void* q, const void* k, const void* vt, const flo
       set_error("corr_warp_fwd: packed fp16 values (vt) are required for this shape (Cv=%d)", Cv);
       return -1;
     }
-    if (Cv <= 0 || Cvp < Cv || (Cvp % 16) != 0 || Cvp > 256) {
-      set_error("corr_warp_fwd: need 0 < Cv <= Cvp <= 256, Cvp %% 16 == 0 (Cv=%d Cvp=%d)", Cv, Cvp);
+    if (Cv <= 0 || Cvp < Cv || (Cvp % 16) != 0) {
+      set_error("corr_warp_fwd: need 0 < Cv <= Cvp, Cvp %% 16 == 0 (Cv=%d Cvp=%d)", Cv, Cvp);
+      return -1;
+    }
+    if (Cvp / VCHUNK > 65535) {
+      set_error("corr_warp_fwd: Cvp=%d needs more than 65535 value chunks of %d", Cvp, VCHUNK);
       return -1;
     }
     if (Nkp < Nk || (Nkp % 8) != 0) {
@@ -319,29 +365,18 @@ int corr_warp_fwd_launch(const void* q, const void* k, const void* vt, const flo
   p.scale = scale;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.out = out; p.lse = lse; p.corr = corr;
-  const int pvn = cuda_pv ? 0 : (Cvp <= 64 ? 64 : Cvp <= 128 ? 128 : 256);
-  // a V stage holds PVN rows of 64 keys (the wgmma reads PVN >= Cvp rows) or Cv fp32 rows of 64 keys
-  p.v_stage = cuda_pv ? 1024 : pvn * BN * 2;
+  p.v_rows = Cvp;
+  p.c0 = 0;
 
-  // shared memory plan (<= 227 KiB): [Q] [K ring] [V ring] [barriers]
-  const int budget = 227 * 1024 - 1024 /*alignment slack*/ - 512 /*barriers*/;
-  p.q_resident = (Kd <= 256) ? 1 : 0;
-  const int q_bytes = p.q_resident ? p.kc_count * Q_ATOM : 0;
-  const int stage = p.q_resident ? K_ATOM : Q_ATOM + K_ATOM;
-  p.ns_v = 2;
-  p.ns_k = (budget - q_bytes - p.ns_v * p.v_stage) / stage;
-  if (p.ns_k > MAX_KSTAGES) p.ns_k = MAX_KSTAGES;
-  if (p.ns_k < 2) {
-    set_error("corr_warp_fwd: shared memory plan failed (Kd=%d Cvp=%d)", Kd, Cvp);
-    return -1;
-  }
-  const int smem_bytes = 1024 + q_bytes + p.ns_k * stage + p.ns_v * p.v_stage + 512;
-
-  CUtensorMap tm_q, tm_k, tm_v;
+  CUtensorMap tm_q, tm_k;
   int rc;
   if ((rc = make_tmap_f16_3d(&tm_q, q, Kd, Nq, B, (uint64_t)Kd * 2, (uint64_t)Nq * Kd * 2, BK, BM, 1))) return rc;
   if ((rc = make_tmap_f16_3d(&tm_k, k, Kd, Nk, B, (uint64_t)Kd * 2, (uint64_t)Nk * Kd * 2, BK, BN, 1))) return rc;
   if (cuda_pv) {
+    p.v_stage = 1024;  // Cv fp32 rows of 64 keys
+    const int smem_bytes = plan_smem(p);
+    if (smem_bytes < 0) return -1;
+    CUtensorMap tm_v;
     if ((rc = make_tmap_f32_3d_plain(&tm_v, v32, Nk, Cv, B, (uint64_t)Nk * 4, (uint64_t)Cv * Nk * 4, BN, Cv, 1)))
       return rc;
     switch (Cv) {
@@ -351,11 +386,13 @@ int corr_warp_fwd_launch(const void* q, const void* k, const void* vt, const flo
       default: return launch_fwd<0, 4>(tm_q, tm_k, tm_v, p, smem_bytes, stream);
     }
   }
-  if ((rc = make_tmap_f16_3d(&tm_v, vt, Nk, Cvp, B, (uint64_t)Nkp * 2, (uint64_t)Cvp * Nkp * 2, BK, Cvp, 1)))
-    return rc;
-  if (pvn == 64) return launch_fwd<64, 0>(tm_q, tm_k, tm_v, p, smem_bytes, stream);
-  if (pvn == 128) return launch_fwd<128, 0>(tm_q, tm_k, tm_v, p, smem_bytes, stream);
-  return launch_fwd<256, 0>(tm_q, tm_k, tm_v, p, smem_bytes, stream);
+  // up to 256 rows: one chunk, grid z = 1.  Beyond: every full chunk of 256 rows in one launch (grid z = chunk), then
+  // the partial last chunk, if any, in a second launch with the PVN that fits it.  Each chunk recomputes S = Q K^T.
+  const int n_full = Cvp > VCHUNK ? Cvp / VCHUNK : 0;
+  const int tail = Cvp - n_full * VCHUNK;
+  if (n_full > 0 && (rc = launch_tensor_pv(tm_q, tm_k, vt, p, Nkp, VCHUNK, 0, n_full, stream))) return rc;
+  if (tail > 0 && (rc = launch_tensor_pv(tm_q, tm_k, vt, p, Nkp, tail, n_full * VCHUNK, 1, stream))) return rc;
+  return 0;
 }
 
 }  // namespace cocos

@@ -759,8 +759,9 @@ def to_op(x, split=False):
 
 
 def attn_chunk(cv):
-    """Value channels per stage-A call of the attend backward: its shared-memory plan takes at most 192 (so 256 value
-    channels -- the adaptor's block, ch = 512 -- run as two calls of 128 whose dS / dS^T the GEMMs add up)."""
+    """Value channels per stage-A call of the attend backward: at most 192, the widest its resident shared-memory plan
+    takes (so 256 value channels -- the adaptor's block, ch = 512 -- run as two calls of 128 whose dS / dS^T the GEMMs
+    add up; stage A's streamed plan for wider calls is used by the module path, corr_bwd.attend_backward)."""
     return round_up(cv, 64) if cv <= 192 else 128
 
 

@@ -57,6 +57,9 @@ int cocos_pack_v_f16(const float* src, void* dst, int B, int Cv, int Nk, int Cvp
  *                                           :362, :368, :370 with operands swapped)
  * q  : fp16 [B, Nq, Kd]   k : fp16 [B, Nk, Kd]   (Kd % 64 == 0)
  * vt : fp16 [B, Cvp, Nkp] (values, channel-major; cocos_pack_v_f16).  May be NULL when v32 is given and Cv <= 4.
+ *      Any Cvp (% 16 == 0): beyond 256 the values run in chunks of 256 rows (the last one may be narrower), each of
+ *      which recomputes the logits and the softmax, so the logit work grows by ceil(Cvp / 256).  Every chunk's
+ *      output is bit for bit what a call on that chunk's channels alone gives; lse and corr come from the first.
  * v32: fp32 [B, Cv, Nk] the same values unpacked (may be NULL).  With Cv <= 4 (the avg-pooled RGB exemplar of
  *      correspondence.py:313-318) the product with the values runs on the CUDA cores inside the exp loop, in fp32.
  * out: fp32 [B, Cv, Nq]   = y.permute(0, 2, 1)  (correspondence.py:323)
@@ -83,7 +86,8 @@ int cocos_gemm_f16(const void* a, const void* b, float* c, int batch, int M, int
  *   dst [B, Nk, Nqp] = ds^T,   pt [B, Nk, Nqp] = P^T (optional, may be NULL)
  * q,k as in cocos_corr_warp_fwd; do16 fp16 [B,Nq,Cvk] = row-scaled upstream gradient
  * dO' = r * dO with rscale = r [B,Nq] (cocos_pack_rows_f16 with rowscale_out), v16 fp16
- * [B,Nk,Cvk] = V position-major (Cvk % 64 == 0); out fp32 [B,Cv,Nq] and lse from the
+ * [B,Nk,Cvk] = V position-major (Cvk % 64 == 0, any width: up to 192 dO and V stay resident in shared memory,
+ * beyond that their 64-channel atoms are streamed; dS is still written once); out fp32 [B,Cv,Nq] and lse from the
  * forward.  The input gradients follow from three bf16 cocos_gemm_f16 calls:
  *   dq^T[Kd,Nq] = k_cm[Kd,Nk] x ds,  dk^T[Kd,Nk] = q_cm[Kd,Nq] x dst,  dv^T[Cv,Nk] = do_cm[Cv,Nq] x pt. */
 int cocos_corr_warp_bwd_ds(const void* q, const void* k, const void* do16, const void* v16, const float* rscale,
@@ -394,7 +398,8 @@ int cocos_nhwc_to_op(const void* x, int x_kind, int Cs, void* y, int y_Cs, int l
  *   vt   fp16 [B, Cvp, Nkp] maxpool2(g) channel-major, K1's V (Cvp % 16 == 0, Nkp % 8 == 0, zero padded)
  * and for the backward (all optional; q_cm and k_cm both or neither):
  *   v16  fp16 [ceil(Cv / Cvk), B, Nk, Cvk] maxpool2(g) position-major in chunks of Cvk channels (Cvk % 64 == 0, zero
- *        beyond Cv): stage A's V, one cocos_corr_warp_bwd_ds call per chunk (its shared-memory plan takes Cvk <= 192)
+ *        beyond Cv): stage A's V, one cocos_corr_warp_bwd_ds call per chunk (the tape keeps Cvk <= 192, where stage A
+ *        keeps dO and V resident)
  *   q_cm bf16 [B, Kd, Nqp], k_cm bf16 [B, Kd, Nkp]: theta and maxpool2(phi) channel-major, the A operands of the
  *        dQ / dK GEMMs (pitches multiples of 8; the padding columns are not written). */
 int cocos_attn_pack_nhwc(const void* z, int z_kind, int z_Cs, int B, int H, int W, int Kd, int Cv, int split, void* q,
