@@ -69,7 +69,7 @@ SIGNATURES = {
                          + [_c_int] * 4 + [_vp, _vp, _vp],
     "cocos_nhwc_to_op": [_vp, _c_int, _c_int, _vp, _c_int, _c_int, _c_ll, _vp],
     "cocos_attn_pack_nhwc": [_vp] + [_c_int] * 8 + [_vp, _vp, _vp, _c_int, _c_int, _vp, _c_int, _vp, _c_int, _vp, _vp],
-    "cocos_attn_do_rows": [_vp] + [_c_int] * 4 + [_vp, _c_int, _vp, _vp, _c_int, _vp, _vp, _vp],
+    "cocos_attn_do_rows": [_vp] + [_c_int] * 4 + [_vp, _c_int, _vp, _vp, _c_int, _vp],
     "cocos_attn_grad_unpack": [_vp] * 4 + [_c_int] * 7 + [_vp, _c_int, _vp],
 }
 

@@ -81,7 +81,7 @@ struct AttnPack {
   uint16_t* k;     // [B, Nk, Kt]  fp16: [hi] or [hi, hi, lo]
   uint16_t* vt;    // [B, Cvp, Nkp] fp16 channel-major
   int Cvp, Nkp;
-  uint16_t* v16;   // [ceil(Cv / Cvk), B, Nk, Cvk] fp16 position-major in chunks of Cvk channels (optional)
+  uint16_t* v16;   // [B, Nk, Cvk] fp16 position-major, zero beyond Cv (optional)
   int Cvk;
   uint16_t* q_cm;  // [B, Kd, Nqp] bf16 (optional)
   int Nqp;
@@ -165,9 +165,8 @@ __global__ void __launch_bounds__(256) attn_kv_kernel(const AttnPack p) {
     }
     return;
   }
-  if (p.v16 != nullptr) {  // [chunk][B][Nk][Cvk]: chunk = channel / Cvk
-    const int cl = cbase + tx, chunk = cl / p.Cvk;
-    uint16_t* dst = p.v16 + (static_cast<size_t>(chunk) * gridDim.z + b) * Nk * p.Cvk + (cl - chunk * p.Cvk);
+  if (p.v16 != nullptr) {  // [B][Nk][Cvk]
+    uint16_t* dst = p.v16 + static_cast<size_t>(b) * Nk * p.Cvk + cbase + tx;
     for (int i = ty; i < TILE; i += 8) {
       const int n = n0 + i;
       if (n < Nk) dst[static_cast<size_t>(n) * p.Cvk] = f16bits(tile[i][tx]);
@@ -180,14 +179,12 @@ __global__ void __launch_bounds__(256) attn_kv_kernel(const AttnPack p) {
 }
 
 // ----------------------------------------------------------------------------------------------- dO rows
-// dy bf16 [B, N, dy_Cs] (Cv channels) -> do16 fp16 [nchunk, B, N, Cvk] = r * dy in chunks of Cvk channels (zero beyond
-// Cv), r = min(1 / max_c |dy|, 2^126) (1 for an all-zero row), do_cm bf16 [B, Cv, Nqp] = dy channel-major and, with more than one
-// chunk, out_ck = K1's output out fp32 [B, Cv, N] regrouped per chunk ([B, cv_chunk, N] each).  32 positions per block,
-// one warp per row for the maxima.
+// dy bf16 [B, N, dy_Cs] (Cv channels) -> do16 fp16 [B, N, Cvk] = r * dy (zero beyond Cv), r = min(1 / max_c |dy|,
+// 2^126) (1 for an all-zero row), and do_cm bf16 [B, Cv, Nqp] = dy channel-major.  32 positions per block, one warp per
+// row for the maxima.
 __global__ void __launch_bounds__(256)
 attn_do_rows_kernel(const uint16_t* __restrict__ dy, int dy_Cs, int N, int Cv, uint16_t* __restrict__ do16, int Cvk,
-                    float* __restrict__ rscale, uint16_t* __restrict__ do_cm, int Nqp, const float* __restrict__ out,
-                    float* __restrict__ out_ck) {
+                    float* __restrict__ rscale, uint16_t* __restrict__ do_cm, int Nqp) {
   __shared__ float tile[TILE][TILE + 1];
   __shared__ float rs[TILE];
   const int b = blockIdx.y, n0 = blockIdx.x * TILE;
@@ -208,8 +205,7 @@ attn_do_rows_kernel(const uint16_t* __restrict__ dy, int dy_Cs, int N, int Cv, u
       if (n < N) rscale[static_cast<size_t>(b) * N + n] = r;
     }
   }
-  const int nchunk = (Cv + Cvk - 1) / Cvk, B = gridDim.y;
-  for (int c0 = 0; c0 < nchunk * Cvk; c0 += TILE) {
+  for (int c0 = 0; c0 < Cvk; c0 += TILE) {
     __syncthreads();
     for (int i = ty; i < TILE; i += 8) {
       const int n = n0 + i, c = c0 + tx;
@@ -217,21 +213,13 @@ attn_do_rows_kernel(const uint16_t* __restrict__ dy, int dy_Cs, int N, int Cv, u
                                       : 0.f;
     }
     __syncthreads();
-    const int chunk = c0 / Cvk, cc0 = c0 - chunk * Cvk;
     for (int i = ty; i < TILE; i += 8) {
       const int n = n0 + i;
-      if (n < N)
-        do16[((static_cast<size_t>(chunk) * B + b) * N + n) * Cvk + cc0 + tx] = f16bits(tile[i][tx] * rs[i]);
+      if (n < N) do16[(static_cast<size_t>(b) * N + n) * Cvk + c0 + tx] = f16bits(tile[i][tx] * rs[i]);
     }
-    const int cvc = min(Cvk, Cv - chunk * Cvk);  // channels of this chunk
     for (int i = ty; i < TILE; i += 8) {
       const int c = c0 + i, n = n0 + tx;
-      if (c < Cv && n < N) {
-        do_cm[(static_cast<size_t>(b) * Cv + c) * Nqp + n] = bf16bits(tile[tx][i]);
-        if (out_ck != nullptr)
-          out_ck[static_cast<size_t>(chunk) * B * Cvk * N + (static_cast<size_t>(b) * cvc + cc0 + i) * N + n] =
-              out[(static_cast<size_t>(b) * Cv + c) * N + n];
-      }
+      if (c < Cv && n < N) do_cm[(static_cast<size_t>(b) * Cv + c) * Nqp + n] = bf16bits(tile[tx][i]);
     }
   }
 }
@@ -345,7 +333,7 @@ int cocos_attn_pack_nhwc(const void* z, int z_kind, int z_Cs, int B, int H, int 
   const long long Nq = static_cast<long long>(H) * W, Nk = Nq / 4;
   if (B <= 0 || H <= 0 || W <= 0 || (H % 2) || (W % 2) || Kd <= 0 || Cv <= 0 || !kind_ok(z_kind) ||
       z_Cs < 2 * Kd + Cv || Cvp < Cv || (Cvp % 16) || Nkp < Nk || (Nkp % 8) || Nqp < Nq || (Nqp % 8) ||
-      (v16 && (Cvk <= 0 || (Cvk % 64))) || (split != 0 && split != 1) || (!q_cm) != (!k_cm)) {
+      (v16 && (Cvk < Cvp || (Cvk % 64))) || (split != 0 && split != 1) || (!q_cm) != (!k_cm)) {
     set_error("cocos_attn_pack_nhwc: bad arguments (B=%d H=%d W=%d Kd=%d Cv=%d z_Cs=%d Cvp=%d Nkp=%d Cvk=%d Nqp=%d)", B,
               H, W, Kd, Cv, z_Cs, Cvp, Nkp, Cvk, Nqp);
     return -1;
@@ -361,29 +349,27 @@ int cocos_attn_pack_nhwc(const void* z, int z_kind, int z_Cs, int B, int H, int 
   const dim3 blk(TILE, 8);
   attn_q_kernel<<<dim3(static_cast<unsigned>(blocks_of(Nq, TILE)), Kp / TILE, B), blk, 0, s>>>(p);
   COCOS_CUDA_CHECK(cudaGetLastError());
-  // V channel tiles up to all chunks of the position-major copy when it is written, else up to Cvp
-  const int vc = v16 ? (Cv + Cvk - 1) / Cvk * Cvk : Cvp;
-  const long long kv_tiles = Kp / TILE + blocks_of(vc, TILE);
+  // V channel tiles up to Cvk when the position-major copy is written (Cvk >= Cvp covers both copies), else up to Cvp
+  const long long kv_tiles = Kp / TILE + blocks_of(v16 ? Cvk : Cvp, TILE);
   attn_kv_kernel<<<dim3(static_cast<unsigned>(blocks_of(Nkp, TILE)), static_cast<unsigned>(kv_tiles), B), blk, 0, s>>>(p);
   COCOS_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
 
 int cocos_attn_do_rows(const void* dy, int dy_Cs, int B, int N, int Cv, void* do16, int Cvk, float* rscale, void* do_cm,
-                       int Nqp, const float* out, float* out_chunks, void* stream) {
-  if (!dy || !do16 || !rscale || !do_cm || (Cvk < Cv && (!out || !out_chunks))) {
+                       int Nqp, void* stream) {
+  if (!dy || !do16 || !rscale || !do_cm) {
     set_error("cocos_attn_do_rows: null pointer argument");
     return -1;
   }
-  if (B <= 0 || N <= 0 || Cv <= 0 || dy_Cs < Cv || Cvk <= 0 || (Cvk % 64) || Nqp < N || (Nqp % 8)) {
+  if (B <= 0 || N <= 0 || Cv <= 0 || dy_Cs < Cv || Cvk < Cv || (Cvk % 64) || Nqp < N || (Nqp % 8)) {
     set_error("cocos_attn_do_rows: bad arguments (B=%d N=%d Cv=%d dy_Cs=%d Cvk=%d Nqp=%d)", B, N, Cv, dy_Cs, Cvk, Nqp);
     return -1;
   }
   attn_do_rows_kernel<<<dim3(static_cast<unsigned>(blocks_of(N, TILE)), B), dim3(TILE, 8), 0,
                         static_cast<cudaStream_t>(stream)>>>(static_cast<const uint16_t*>(dy), dy_Cs, N, Cv,
                                                              static_cast<uint16_t*>(do16), Cvk, rscale,
-                                                             static_cast<uint16_t*>(do_cm), Nqp, out,
-                                                             Cvk < Cv ? out_chunks : nullptr);
+                                                             static_cast<uint16_t*>(do_cm), Nqp);
   COCOS_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

@@ -302,7 +302,7 @@ def _adaptor_blocks(net):
 
 def attention_supported(attn):
     """The SAGAN block on the tape (T.attention): four plain bias-free 1x1 convolutions without forward pre-hooks (no
-    spectral norm) and at most 256 value channels (K1's limit)."""
+    spectral norm) and at most 256 value channels, the widest the tape is tested at."""
     convs = (attn.theta, attn.phi, attn.g, attn.o)
     plain = all(isinstance(c, nn.Conv2d) and c.kernel_size == (1, 1) and c.stride == (1, 1) and c.padding == (0, 0)
                 and c.dilation == (1, 1) and c.groups == 1 and c.bias is None and c.padding_mode == "zeros"

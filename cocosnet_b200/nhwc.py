@@ -329,7 +329,7 @@ class NativeBackend:
     def attn_pack(self, z, kd, cv, split, q, k, vt, v16, q_cm, k_cm):
         _lib.check(self.lib.cocos_attn_pack_nhwc(
             z.t.data_ptr(), z.kind, z.Cs, z.B, z.H, z.W, kd, cv, int(split), q.data_ptr(), k.data_ptr(), vt.data_ptr(),
-            vt.shape[1], vt.stride(1), _p(v16), v16.shape[3] if v16 is not None else 0, _p(q_cm),
+            vt.shape[1], vt.stride(1), _p(v16), v16.shape[2] if v16 is not None else 0, _p(q_cm),
             q_cm.stride(1) if q_cm is not None else round_up(z.H * z.W, 8), _p(k_cm), _stream()),
             "cocos_attn_pack_nhwc", kernels=2)
 
@@ -342,14 +342,14 @@ class NativeBackend:
         from . import ops
         return ops.corr_warp_bwd_ds(q, k, do16, rscale, v16, out, lse, cv, 1.0, want_pt)
 
-    def gemm(self, a, b, out=None):
+    def gemm(self, a, b):
         from . import ops
-        return ops.gemm_f16(a, b, out=out, accumulate=out is not None)
+        return ops.gemm_f16(a, b)
 
-    def attn_do_rows(self, dy, cv, do16, rscale, do_cm, out, out_ck):
+    def attn_do_rows(self, dy, cv, do16, rscale, do_cm):
         _lib.check(self.lib.cocos_attn_do_rows(dy.t.data_ptr(), dy.Cs, dy.B, dy.H * dy.W, cv, do16.data_ptr(),
-                                               do16.shape[3], rscale.data_ptr(), do_cm.data_ptr(), do_cm.stride(1),
-                                               out.data_ptr(), _p(out_ck), _stream()), "cocos_attn_do_rows")
+                                               do16.shape[2], rscale.data_ptr(), do_cm.data_ptr(), do_cm.stride(1),
+                                               _stream()), "cocos_attn_do_rows")
 
     def attn_grad_unpack(self, dq, dk, dv, z, kd, cv, dz):
         _lib.check(self.lib.cocos_attn_grad_unpack(dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), z.t.data_ptr(), z.kind,
@@ -758,13 +758,6 @@ def to_op(x, split=False):
     return y
 
 
-def attn_chunk(cv):
-    """Value channels per stage-A call of the attend backward: at most 192, the widest its resident shared-memory plan
-    takes (so 256 value channels -- the adaptor's block, ch = 512 -- run as two calls of 128 whose dS / dS^T the GEMMs
-    add up; stage A's streamed plan for wider calls is used by the module path, corr_bwd.attend_backward)."""
-    return round_up(cv, 64) if cv <= 192 else 128
-
-
 def attn_pack(z, kd, cv, split=False, for_backward=True):
     """Raw output z of the theta | phi | g 1x1 convolution (channels [0, kd) theta, [kd, 2kd) phi, [2kd, 2kd + cv) g)
     -> (q, k, vt, saved): K1's operands -- theta rows, maxpool2(phi) rows (3-term split layouts when `split`) and
@@ -780,8 +773,7 @@ def attn_pack(z, kd, cv, split=False, for_backward=True):
     vt = be.empty((z.B, round_up(cv, 16), round_up(nk, 8)), F16, dev)
     v16 = q_cm = k_cm = None
     if for_backward:
-        cvk = attn_chunk(cv)
-        v16 = be.empty(((cv + cvk - 1) // cvk, z.B, nk, cvk), F16, dev)
+        v16 = be.empty((z.B, nk, round_up(cv, 64)), F16, dev)
         q_cm = be.empty((z.B, kd, round_up(nq, 8)), BF16, dev)[:, :, :nq]
         k_cm = be.empty((z.B, kd, round_up(nk, 8)), BF16, dev)[:, :, :nk]
     be.attn_pack(z, kd, cv, split, q, k, vt, v16, q_cm, k_cm)
@@ -801,21 +793,12 @@ def attend_backward(dy, z, kd, cv, q, k, out, lse, saved):
     be, dev = backend(), dy.t.device
     v16, q_cm, k_cm = saved
     nq = dy.H * dy.W
-    cvk = v16.shape[3]
-    nchunk = v16.shape[0]
-    do16 = be.empty((nchunk, dy.B, nq, cvk), F16, dev)
+    do16 = be.empty((dy.B, nq, v16.shape[2]), F16, dev)
     rscale = torch.empty((dy.B, nq), dtype=torch.float32, device=dev)
     do_cm = be.empty((dy.B, cv, round_up(nq, 8)), BF16, dev)[:, :, :nq]
-    out_ck = torch.empty((nchunk * dy.B * cvk * nq,), dtype=torch.float32, device=dev) if nchunk > 1 else None
-    be.attn_do_rows(dy, cv, do16, rscale, do_cm, out, out_ck)
-    dq = dk = dv = None
-    for c in range(nchunk):  # dS is linear in the value channels: the chunks' dS / dS^T add up in the GEMMs
-        cvc = min(cvk, cv - c * cvk)
-        oc = out if nchunk == 1 else out_ck[c * dy.B * cvk * nq:][:dy.B * cvc * nq].view(dy.B, cvc, nq)
-        ds, dst, pt = be.attend_bwd_ds(q, k, do16[c], rscale, v16[c], oc, lse, cvc, want_pt=c == 0)
-        dq, dk = be.gemm(k_cm, ds, out=dq), be.gemm(q_cm, dst, out=dk)
-        if c == 0:
-            dv = be.gemm(do_cm, pt)
+    be.attn_do_rows(dy, cv, do16, rscale, do_cm)
+    ds, dst, pt = be.attend_bwd_ds(q, k, do16, rscale, v16, out, lse, cv, want_pt=True)
+    dq, dk, dv = be.gemm(k_cm, ds), be.gemm(q_cm, dst), be.gemm(do_cm, pt)
     dz = new(z.B, z.H, z.W, z.C, BF16, dev, zero=False)
     be.attn_grad_unpack(dq, dk, dv, z, kd, cv, dz)
     return dz

@@ -20,7 +20,7 @@
 extern "C" {
 #endif
 
-#define COCOS_ABI_VERSION 7
+#define COCOS_ABI_VERSION 8
 
 /* Multi-block reductions (cocos_conv_wgrad, cocos_tapwgrad, cocos_sn_power_iter, cocos_in_stats_nhwc,
  * cocos_inst_act_nhwc_bwd, cocos_pair_loss_nhwc_fwd, cocos_colsum_nhwc, cocos_se_nhwc_fwd / _bwd) write one partial sum per block into a
@@ -397,23 +397,20 @@ int cocos_nhwc_to_op(const void* x, int x_kind, int Cs, void* y, int y_Cs, int l
  *   k    fp16 [B, Nk, Kt]  maxpool2(phi) rows: [hi] or the key layout [hi, hi, lo]
  *   vt   fp16 [B, Cvp, Nkp] maxpool2(g) channel-major, K1's V (Cvp % 16 == 0, Nkp % 8 == 0, zero padded)
  * and for the backward (all optional; q_cm and k_cm both or neither):
- *   v16  fp16 [ceil(Cv / Cvk), B, Nk, Cvk] maxpool2(g) position-major in chunks of Cvk channels (Cvk % 64 == 0, zero
- *        beyond Cv): stage A's V, one cocos_corr_warp_bwd_ds call per chunk (the tape keeps Cvk <= 192, where stage A
- *        keeps dO and V resident)
+ *   v16  fp16 [B, Nk, Cvk] maxpool2(g) position-major (Cvk >= Cvp, Cvk % 64 == 0, zero beyond Cv): stage A's V, one
+ *        cocos_corr_warp_bwd_ds call at any Cvk
  *   q_cm bf16 [B, Kd, Nqp], k_cm bf16 [B, Kd, Nkp]: theta and maxpool2(phi) channel-major, the A operands of the
  *        dQ / dK GEMMs (pitches multiples of 8; the padding columns are not written). */
 int cocos_attn_pack_nhwc(const void* z, int z_kind, int z_Cs, int B, int H, int W, int Kd, int Cv, int split, void* q,
                          void* k, void* vt, int Cvp, int Nkp, void* v16, int Cvk, void* q_cm, int Nqp, void* k_cm,
                          void* stream);
 /* dO rows of the attend backward from dy, the bf16 NHWC gradient of the attention output ([B, N, dy_Cs], Cv channels;
- * the gradient of bmm(g, beta^T) in architecture.py:126): do16 fp16 [ceil(Cv / Cvk), B, N, Cvk] = r * dy in chunks of
- * Cvk channels (Cvk % 64 == 0, zero beyond Cv) with r = min(1 / max_c |dy|, 2^126) over all Cv channels (1 for an all-zero row)
- * written to rscale [B, N] -- what cocos_pack_rows_f16 with rowscale_out makes from fp32 channel-major -- and do_cm
- * bf16 [B, Cv, Nqp] = dy channel-major, the A operand of the dV GEMM.  With more than one chunk, out_chunks receives
- * K1's output out fp32 [B, Cv, N] regrouped per chunk (chunk c: [B, cv_c, N] at offset c * B * Cvk * N), the `out`
- * of each stage-A call; otherwise out / out_chunks may be NULL. */
+ * the gradient of bmm(g, beta^T) in architecture.py:126): do16 fp16 [B, N, Cvk] = r * dy (Cvk >= Cv, Cvk % 64 == 0,
+ * zero beyond Cv) with r = min(1 / max_c |dy|, 2^126) (1 for an all-zero row) written to rscale [B, N] -- what
+ * cocos_pack_rows_f16 with rowscale_out makes from fp32 channel-major -- and do_cm bf16 [B, Cv, Nqp] = dy
+ * channel-major, the A operand of the dV GEMM. */
 int cocos_attn_do_rows(const void* dy, int dy_Cs, int B, int N, int Cv, void* do16, int Cvk, float* rscale, void* do_cm,
-                       int Nqp, const float* out, float* out_chunks, void* stream);
+                       int Nqp, void* stream);
 /* Gradient of the theta | phi | g output from the three GEMM results dq fp32 [B, Kd, Nq], dk fp32 [B, Kd, Nk], dv fp32
  * [B, Cv, Nk] (channel-major, dense): dz bf16 [B, H, W, dz_Cs] (fully overwritten, zero beyond 2Kd + Cv) with theta's
  * channels = dq transposed and phi's / g's = dk / dv at the first maximum in scan order of each 2x2 window of z, zero

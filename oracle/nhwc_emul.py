@@ -423,11 +423,9 @@ class EmulBackend:
         full = torch.zeros(vt.shape)
         full[:, :cv, :nk] = g.transpose(1, 2)
         vt.copy_(self._round(full, F16).to(vt.dtype))
-        if v16 is not None:  # [chunk, B, Nk, cvk]
-            nch, cvk = v16.shape[0], v16.shape[3]
-            full = torch.zeros(B, nk, nch * cvk)
+        if v16 is not None:  # [B, Nk, Cvk], zero beyond cv
+            full = torch.zeros(v16.shape)
             full[..., :cv] = g
-            full = full.reshape(B, nk, nch, cvk).permute(2, 0, 1, 3)
             v16.copy_(self._round(full, F16).to(v16.dtype))
         if q_cm is not None:
             q_cm.copy_(self._round(theta.transpose(1, 2), BF16).to(q_cm.dtype))
@@ -453,26 +451,20 @@ class EmulBackend:
         bf = lambda t: self._round(t, BF16).to(self.dtype(BF16))  # noqa: E731
         return bf(ds), bf(ds.transpose(1, 2)), (bf(p.transpose(1, 2)) if want_pt else None)
 
-    def gemm(self, a, b, out=None):
-        c = a.float() @ b.float().transpose(1, 2)
-        return c if out is None else out.add_(c)
+    def gemm(self, a, b):
+        return a.float() @ b.float().transpose(1, 2)
 
-    def attn_do_rows(self, dy, cv, do16, rscale, do_cm, out, out_ck):
+    def attn_do_rows(self, dy, cv, do16, rscale, do_cm):
         B, N = dy.B, dy.H * dy.W
         d = dy.t.float()[..., :cv].reshape(B, N, cv)
         m = d.abs().amax(2)
         # capped at 2^126 like the kernel: 1/m overflows fp32 for a subnormal maximum m <= 2^-128
         r = torch.where((m > 0) & torch.isfinite(m), (1.0 / m).clamp_max(2.0 ** 126), torch.ones_like(m))
         rscale.copy_(r)
-        nch, cvk = do16.shape[0], do16.shape[3]
-        full = torch.zeros(B, N, nch * cvk)
+        full = torch.zeros(do16.shape)
         full[..., :cv] = d * r[..., None]
-        do16.copy_(self._round(full.reshape(B, N, nch, cvk).permute(2, 0, 1, 3), F16).to(do16.dtype))
+        do16.copy_(self._round(full, F16).to(do16.dtype))
         do_cm.copy_(d.transpose(1, 2).to(do_cm.dtype))
-        if out_ck is not None:  # chunk c: out[:, c*cvk : c*cvk + cv_c] as [B, cv_c, N] at offset c * B * cvk * N
-            for c in range(nch):
-                part = out[:, c * cvk:min(cv, (c + 1) * cvk)]
-                out_ck[c * B * cvk * N:][:part.numel()].copy_(part.reshape(-1))
 
     def attn_grad_unpack(self, dq, dk, dv, z, kd, cv, dz):
         B, H, W = z.B, z.H, z.W

@@ -4,7 +4,7 @@ import os
 import re
 
 
-def test_header_symbols_exported():
+def test_header_symbols_and_abi_version():
     from cocosnet_b200 import _lib
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     if not os.path.exists(_lib.LIB_PATH):
@@ -16,7 +16,7 @@ def test_header_symbols_exported():
     for name in declared:
         assert hasattr(h, name), name
     assert declared == set(_lib.SIGNATURES), (declared ^ set(_lib.SIGNATURES))
-    assert h.cocos_abi_version() == 7
+    assert h.cocos_abi_version() == 8
 
 
 def test_ctypes_signatures_match_header_arity_and_kinds():
@@ -52,3 +52,10 @@ def test_bad_arguments_are_errors_not_crashes():
     assert h.cocos_corr_warp_fwd(None, None, None, None, None, None, None, 1, 1, 1, 64, 3, 16, 8, 1.0, None) != 0
     assert b"null" in h.cocos_last_error()
     assert h.cocos_pack_rows_f16(None, None, 0, 1, 1, 2, 0, None, None) != 0
+    # the attention's position-major V and dO rows hold every value channel in one row: Cvk narrower than Cv is refused
+    # (non-null dummy pointers: nothing is dereferenced before the check)
+    assert h.cocos_attn_pack_nhwc(16, 3, 384, 1, 8, 8, 64, 256, 0, 16, 16, 16, 256, 16, 16, 128, None, 64, None,
+                                  None) != 0
+    assert b"bad arguments" in h.cocos_last_error()
+    assert h.cocos_attn_do_rows(16, 256, 1, 64, 256, 16, 128, 16, 16, 64, None) != 0
+    assert b"bad arguments" in h.cocos_last_error()

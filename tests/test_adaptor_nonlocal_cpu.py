@@ -66,7 +66,7 @@ def emul(request):
 NAMES = ("y", "x", "theta", "phi", "g", "o", "gamma")
 
 
-@pytest.mark.parametrize("shape", [(64, 8, 6), (128, 4, 12), (512, 4, 4)])  # 512: two stage-A chunks of 128
+@pytest.mark.parametrize("shape", [(64, 8, 6), (128, 4, 12), (512, 4, 4)])  # 512: the adaptor's 256 value channels
 def test_attention_matches_the_module_in_fp64(emul, shape):
     ch, H, W = shape
     m, x, gy = attention_case(ch, H, W)

@@ -575,28 +575,21 @@ def fp64_attend(q, k, v, d_out, s):
     return out.detach(), q.grad, k.grad, v.grad
 
 
-def e2e_bounds(q16, k16, V, dO, s, cuda_pv, chunk=None):
+def e2e_bounds(q16, k16, V, dO, s, cuda_pv):
     """Bounds of dq [B,Kd,Nq], dk [B,Kd,Nk], dv [B,Cv,Nk] of the attend backward, carried through stage A and the
-    GEMMs; dO [B,Nq,Cv] the exact upstream gradient.  With `chunk`, stage A runs per chunk of value channels: each
-    chunk's dS is rounded to bf16 on its own and the GEMMs add the chunks up."""
+    GEMMs; dO [B,Nq,Cv] the exact upstream gradient."""
     r = fwd_reference(q16, k16, V, s)
     ob, lb, _ = fwd_bounds(r, cuda_pv)
     P = r["Ph"] / r["l"]
     Vd = r["V"].transpose(1, 2)                                      # [B,Nk,Cv]
     e = r["e"][..., None] + lb[..., None]                            # P's budget: the logits and lse
-    cv = Vd.shape[2]
-    dsb = own = 0
-    for c0 in range(0, cv, chunk or cv):
-        sl = slice(c0, c0 + (chunk or cv))
-        dP = dO[..., sl] @ Vd[..., sl].transpose(1, 2)
-        D = (dO[..., sl] * r["O"][..., sl]).sum(2, keepdim=True)
-        dS = s * P * (dP - D)
-        acc = dO[..., sl].abs() @ Vd[..., sl].abs().transpose(1, 2) + \
-            (dO[..., sl].abs() * r["O"][..., sl].abs()).sum(2, keepdim=True)
-        dsb = dsb + ulp(dS, "bf16") + 2.0 ** -21 * dS.abs() + s * P * (
-            (2.0 ** -16 + 2.0 ** -11) * acc + (dO[..., sl].abs() * ob[..., sl]).sum(2, keepdim=True)
-            + 2 * e * (dP - D).abs())
-        own = own + 2.0 ** -16 * dS.abs()
+    dP = dO @ Vd.transpose(1, 2)
+    D = (dO * r["O"]).sum(2, keepdim=True)
+    dS = s * P * (dP - D)
+    acc = dO.abs() @ Vd.abs().transpose(1, 2) + (dO.abs() * r["O"].abs()).sum(2, keepdim=True)
+    dsb = ulp(dS, "bf16") + 2.0 ** -21 * dS.abs() + s * P * (
+        (2.0 ** -16 + 2.0 ** -11) * acc + (dO.abs() * ob).sum(2, keepdim=True) + 2 * e * (dP - D).abs())
+    own = 2.0 ** -16 * dS.abs()
     Q, K = q16.double(), k16.double()
     gq = K.abs().transpose(1, 2) @ (dsb + own).transpose(1, 2)      # [B,Kd,Nq]
     gk = Q.abs().transpose(1, 2) @ (dsb + own)                      # [B,Kd,Nk]
@@ -634,18 +627,18 @@ def test_corr_attend_forward_backward_per_element(name, B, N, C, Cv, s):
     print("attend %-30s worst err/bound out %.3g dq %.3g dk %.3g dv %.3g" % ((name,) + tuple(w)))
 
 
-def test_nhwc_attend_two_stage_a_chunks_per_element():
-    """nhwc.attend / nhwc.attend_backward at cv = 256 (two stage-A chunks of 128 whose dS add up in the GEMMs, split
-    Q / K) against fp64 autograd through the 2x2 max pooling, on bf16- and fp16-exact z and dy."""
+def test_nhwc_attend_one_streamed_stage_a_call_per_element():
+    """nhwc.attend / nhwc.attend_backward at cv = 256 (one stage-A call on its streamed plan, split Q / K) against
+    fp64 autograd through the 2x2 max pooling, on bf16- and fp16-exact z and dy."""
     import torch.nn.functional as F
     dev = "cuda"
     B, H, W, kd, cv = 1, 16, 12, 64, 256
-    assert nhwc.attn_chunk(cv) == 128
     g = torch.Generator().manual_seed(5)
     z = exact16(torch.randn(B, 2 * kd + cv, H, W, generator=g) * 0.5)
     dy = exact16(torch.randn(B, cv, H, W, generator=g))
     zn = nhwc.pack(z.to(dev), nhwc.F32)
     q, k, vt, saved = nhwc.attn_pack(zn, kd, cv, split=True)
+    assert saved[0].shape[2] == 256  # Cvk > 192: stage A streams dO and V through its operand ring
     out, lse = nhwc.attend(q, k, vt, cv)
     dz = nhwc.attend_backward(nhwc.pack(dy.to(dev), nhwc.BF16), zn, kd, cv, q, k, out, lse, saved)
     torch.cuda.synchronize()
@@ -657,8 +650,7 @@ def test_nhwc_attend_two_stage_a_chunks_per_element():
     o = (P @ gv.transpose(1, 2)).transpose(1, 2)
     o.backward(dy.to(dev).double().reshape(B, cv, -1))
     V = vt[:, :cv, :k.shape[1]]
-    gq, gk, gvb, ob, _ = e2e_bounds(q, k, V, dy.to(dev).double().reshape(B, cv, -1).transpose(1, 2), 1.0, False,
-                                    chunk=nhwc.attn_chunk(cv))
+    gq, gk, gvb, ob, _ = e2e_bounds(q, k, V, dy.to(dev).double().reshape(B, cv, -1).transpose(1, 2), 1.0, False)
     w_out = check(out.transpose(1, 2), o.detach().transpose(1, 2), ob, "nhwc out")
     # the bounds of dq | dk | dv routed through the pooling like the gradients, then the bf16 rounding of dz
     bq, bk = gq[:, :kd], gk[:, :kd]  # the GEMMs contract the bf16 channel-major theta / phi: the hi segments
@@ -670,4 +662,4 @@ def test_nhwc_attend_two_stage_a_chunks_per_element():
     bound = bound + ulp(ref, "bf16") + 2.0 ** -8 * bound
     got = dz.t[..., :2 * kd + cv].permute(0, 3, 1, 2)
     w_dz = check(got, ref, bound, "nhwc dz")
-    print("nhwc attend cv256 two chunks: worst err/bound out %.3g dz %.3g" % (w_out, w_dz))
+    print("nhwc attend cv256 one stage-A call: worst err/bound out %.3g dz %.3g" % (w_out, w_dz))

@@ -84,10 +84,11 @@ from tests.test_gpu_adaptor_variants import (  # noqa: E402,F401
     test_dilated_tapconv_forward_dgrad_wgrad, test_se_forward_backward_match_fp64_autograd_and_repeat_bitwise,
     test_wide_halos_through_every_writer_and_fold)
 from tests.test_gpu_adaptor_nonlocal import (  # noqa: E402,F401
-    test_attention_at_gamma_zero_on_the_gpu, test_attention_matches_fp64_autograd, test_new_kernels_match_their_emulation)
+    test_attention_at_gamma_zero_on_the_gpu, test_attention_layout_kernels_match_their_emulation,
+    test_attention_matches_fp64_autograd)
 from tests.test_gpu_attend_edges import (  # noqa: E402,F401
     test_corr_attend_forward_backward_per_element, test_gemm_per_element, test_k1_forward_per_element,
-    test_nhwc_attend_two_stage_a_chunks_per_element, test_stage_a_per_element)
+    test_nhwc_attend_one_streamed_stage_a_call_per_element, test_stage_a_per_element)
 from tests.test_gpu_model import test_train_step_matches_reference_golden  # noqa: E402,F401
 
 

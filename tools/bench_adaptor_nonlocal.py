@@ -29,7 +29,7 @@ ATTN_SHAPES = {"generator_256x128": (256, 128), "discriminator_256x32": (256, 32
 
 
 def timed(run, paths, warmup, reps):
-    """run(path, events | None) -> False when it ran the forward only; returns {path: {"fwd": [...], "bwd": [...]}} from alternated runs."""
+    """run(path, events | None); returns {path: {"fwd": [...], "bwd": [...]}} from alternated runs."""
     for p in paths:
         for _ in range(warmup):
             run(p)
@@ -38,11 +38,10 @@ def timed(run, paths, warmup, reps):
     for r in range(reps):
         for p in (paths if r % 2 == 0 else paths[::-1]):
             ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
-            timed_bwd = run(p, ev) is not False  # False: forward only (the path's backward fails)
+            run(p, ev)
             torch.cuda.synchronize()
             times[p]["fwd"].append(ev[0].elapsed_time(ev[1]))
-            if timed_bwd:
-                times[p]["bwd"].append(ev[1].elapsed_time(ev[2]))
+            times[p]["bwd"].append(ev[1].elapsed_time(ev[2]))
     return times
 
 
@@ -67,7 +66,7 @@ def bench_adaptor(a):
         net.attn.gamma.fill_(0.5)  # a trained block: the attention reaches the output and every weight gets a gradient
     g = torch.Generator(device="cuda").manual_seed(0)
     x = torch.randn(a.batch, 3, a.size, a.size, device="cuda", generator=g)
-    taken, bwd_error = [0], {}
+    taken = [0]
     real = T.attention
 
     def counting(*args, **kw):
@@ -87,13 +86,7 @@ def bench_adaptor(a):
             events[1].record()
         if "g" not in gy:
             gy["g"] = torch.randn(y.shape, device="cuda", generator=g)
-        if path in bwd_error:
-            return False
-        try:
-            y.backward(gy["g"])
-        except RuntimeError as e:  # the module path's attend backward takes at most 192 value channels
-            bwd_error[path] = str(e).splitlines()[0]
-            return False
+        y.backward(gy["g"])
         if events:
             events[2].record()
 
@@ -103,20 +96,7 @@ def bench_adaptor(a):
     os.environ["COCOS_NHWC"] = "0"
     assert not fast.adaptor_supported(net, x)
     paths = ["tape", "module"]
-    times = timed(run, paths, a.warmup, a.reps)
-    if not bwd_error:
-        return summary(times, paths)
-    # a path whose backward fails is timed forward only
-    med = lambda v: sorted(v)[len(v) // 2]  # noqa: E731
-    res = {p: {"fwd_ms": med(times[p]["fwd"]), "fwd_ms_all": [round(t, 3) for t in times[p]["fwd"]]} for p in paths}
-    for p in paths:
-        if p in bwd_error:
-            res[p]["bwd_error"] = bwd_error[p]
-        else:
-            res[p]["bwd_ms"] = med(times[p]["bwd"])
-            res[p]["fwd_bwd_ms"] = med([f + b for f, b in zip(times[p]["fwd"], times[p]["bwd"])])
-    res["module_over_tape_fwd"] = res["module"]["fwd_ms"] / res["tape"]["fwd_ms"]
-    return res
+    return summary(timed(run, paths, a.warmup, a.reps), paths)
 
 
 def bench_attention(a, ch, h):
